@@ -36,8 +36,8 @@ class Bucket(C.Structure):
 class BlockedPairs(C.Structure):
     _fields_ = [
         ("n_pools", C.c_int64), ("n_tiles", C.c_int64), ("pools_per_tile", C.c_int32), ("reserved", C.c_int32),
-        ("r0", C.c_void_p), ("r1", C.c_void_p), ("gamma_inv", C.c_void_p), ("lid", C.c_void_p),
-        ("pos", C.c_void_p), ("rows", C.c_void_p), ("tok", C.c_void_p), ("desc", C.c_void_p),
+        ("r0", C.c_void_p), ("r1", C.c_void_p), ("gamma_inv", C.c_void_p), ("pw", C.c_void_p),
+        ("reserved_ptr", C.c_void_p), ("rows", C.c_void_p), ("tok", C.c_void_p), ("desc", C.c_void_p),
     ]
 
 

@@ -31,7 +31,7 @@ k_blocked(const BlockedArgs A) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Variant "regs" (configuration 3): the per-pool slabs (R0, R1, 1/gamma, ids, positions) are read exactly once, so they
+// Variant "regs" (configuration 3): the per-pool slabs (R0, R1, 1/gamma, pool words) are read exactly once, so they
 // go global -> registers directly (coalesced LDG, prefetched one tile ahead) instead of through shared memory.  Only
 // the small per-tile tables (row table, token list, descriptor) ride a 4-deep TMA ring.  That frees ~80 KB of shared
 // memory per CTA, which pays for double-buffered nu_local and flows, and those allow ONE barrier per tile: the row
@@ -59,7 +59,7 @@ __device__ __forceinline__ void issue_tables(TabStage<P>* st, uint64_t* bar, con
 template <int NF>
 struct PoolRegs {
     double a[NF];
-    uint32_t lid, pos;
+    uint32_t pw;
 };
 
 template <int P, int THREADS, int NF, int NPOOL>
@@ -70,20 +70,18 @@ __device__ __forceinline__ void load_pools(PoolRegs<NF> (&r)[NPOOL], const Block
         const long long q = toff + tid + u * THREADS;
 #pragma unroll
         for (int k = 0; k < NF; ++k) r[u].a[k] = __ldg(A.slab[k] + q);
-        r[u].lid = __ldg(A.lid + q);
-        r[u].pos = __ldg(A.pos + q);
+        r[u].pw = __ldg(A.pw + q);
     }
 }
 
-// pull the slabs of `tile` from HBM into L2 ahead of the register loads (one thread, 5 bulk prefetches)
+// pull the slabs of `tile` from HBM into L2 ahead of the register loads (one thread, NF + 1 bulk prefetches)
 template <int P, int NF>
 __device__ __forceinline__ void prefetch_pools_l2(const BlockedArgs& A, long long tile) {
     constexpr int tp = P;
     const long long toff = tile * P;
 #pragma unroll
     for (int k = 0; k < NF; ++k) bulk_prefetch_l2(A.slab[k] + toff, tp * 8);
-    bulk_prefetch_l2(A.lid + toff, tp * 4);
-    bulk_prefetch_l2(A.pos + toff, tp * 4);
+    bulk_prefetch_l2(A.pw + toff, tp * 4);
 }
 
 template <int P, int THREADS, int STAGES, int MODE, bool TRADES, bool HESS>
@@ -96,7 +94,7 @@ k_blocked_regs(const BlockedArgs A) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     St* stages = reinterpret_cast<St*>(smem_raw);
     double* nul0 = reinterpret_cast<double*>(smem_raw + (size_t)STAGES * sizeof(St));      // [2][P]  nu_local
-    double* g0 = nul0 + 2 * P;                                                              // [2][2P] flows, row order
+    double* g0 = nul0 + 2 * P;                                                              // [2][2P] flows
     __shared__ uint64_t full[STAGES];
     __shared__ double part[THREADS / 32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -155,18 +153,18 @@ k_blocked_regs(const BlockedArgs A) {
                 }
             }
         }
-        // 2. pool phase of this tile (registers + nu_local) -> flows in row order
+        // 2. pool phase of this tile (registers + nu_local) -> flows
         {
             double f0[NPOOL], f1[NPOOL];
 #pragma unroll
             for (int u = 0; u < NPOOL; ++u) {
-                const uint32_t li = cur[u].lid;
+                const uint32_t w = cur[u].pw;
                 if (MODE == 0) {
                     EvalOp::apply<TRADES, HESS>(A, tile * P + tid + u * THREADS, cur[u].a[0], cur[u].a[NF > 1 ? 1 : 0],
-                                                cur[u].a[NF > 2 ? 2 : 0], nul[li & 0xffffu], nul[li >> 16], f0[u], f1[u],
+                                                cur[u].a[NF > 2 ? 2 : 0], nul[pw_lid0(w)], nul[pw_lid1(w)], f0[u], f1[u],
                                                 acc);
                 } else if (MODE == 1) {
-                    f0[u] = cur[u].a[0] * (nul[li & 0xffffu] - nul[li >> 16]);
+                    f0[u] = cur[u].a[0] * (nul[pw_lid0(w)] - nul[pw_lid1(w)]);
                     f1[u] = -f0[u];
                 } else {
                     f0[u] = cur[u].a[0];
@@ -175,8 +173,8 @@ k_blocked_regs(const BlockedArgs A) {
             }
 #pragma unroll
             for (int u = 0; u < NPOOL; ++u) {
-                g[cur[u].pos & 0xffffu] = f0[u];
-                g[cur[u].pos >> 16] = f1[u];
+                g[tid + u * THREADS] = f0[u];
+                g[P + pw_pos1(cur[u].pw)] = f1[u];
             }
         }
         // 3. nu_local of the next tile into the other buffer (read last in the pool phase of tile-1: before barrier-1)
@@ -228,17 +226,17 @@ k_blocked_regs(const BlockedArgs A) {
 }
 
 // dense assembly (small-n direct solves of mixed problems): H += sum_i A_i h_i [[1,-1],[-1,1]] A_i' straight from the blocked
-// layout -- the pool's global tokens are its tile's token list at its 16-bit local ids
+// layout -- the pool's global tokens are its tile's token list at the local ids of its pool word
 __global__ void __launch_bounds__(256)
-k_blocked_dense(long long n_pools, int n, const uint32_t* __restrict__ lid, const int32_t* __restrict__ tok,
+k_blocked_dense(long long n_pools, int n, const uint32_t* __restrict__ pw, const int32_t* __restrict__ tok,
                 const double* __restrict__ hcoef, double* H) {
     for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n_pools; q += (long long)gridDim.x * blockDim.x) {
         const double h = hcoef[q];
         if (h != 0.0) {
             const long long tile = q / kTileP;
-            const uint32_t li = lid[q];
-            const long long a = tok[tile * BlockedCfg<kTileP>::kTokMax + (li & 0xffffu)];
-            const long long b = tok[tile * BlockedCfg<kTileP>::kTokMax + (li >> 16)];
+            const uint32_t w = pw[q];
+            const long long a = tok[tile * BlockedCfg<kTileP>::kTokMax + pw_lid0(w)];
+            const long long b = tok[tile * BlockedCfg<kTileP>::kTokMax + pw_lid1(w)];
             atomicAdd(H + a * n + a, h); atomicAdd(H + b * n + b, h);
             atomicAdd(H + a * n + b, -h); atomicAdd(H + b * n + a, -h);
         }
@@ -303,10 +301,11 @@ int fill_blocked_args(const cfmm_blocked_pairs* b, BlockedArgs& A) {
     if (!b) return CFMM_E_NULL;
     if (b->pools_per_tile != kTileP) return CFMM_E_KIND;          // layout built for another library version
     if (b->n_tiles < 0 || b->n_pools < 0 || b->n_pools > b->n_tiles * (int64_t)kTileP) return CFMM_E_SIZE;
-    if (b->n_tiles > 0 && (!b->lid || !b->pos || !b->rows || !b->tok || !b->desc)) return CFMM_E_NULL;
+    if (b->reserved_ptr) return CFMM_E_KIND;                       // a separate position array: layout of an older library
+    if (b->n_tiles > 0 && (!b->pw || !b->rows || !b->tok || !b->desc)) return CFMM_E_NULL;
     A.n_tiles = b->n_tiles;
     A.M = b->n_tiles * (int64_t)kTileP;                            // slab stride (= where slot 1 of delta / lambda starts)
-    A.lid = b->lid; A.pos = b->pos; A.rows = b->rows; A.tok = b->tok;
+    A.pw = b->pw; A.rows = b->rows; A.tok = b->tok;
     A.desc = reinterpret_cast<const int4*>(b->desc);
     A.zero_next = nullptr; A.n_zero = 0;
     A.slab[0] = A.slab[1] = A.slab[2] = nullptr;
@@ -379,7 +378,7 @@ int cfmm_blocked_dense(const cfmm_blocked_pairs* b, int32_t n_tokens, const doub
     // (pools of the padded tail carry hcoef = 0: the evaluation writes 0 for them)
     const long long total = b->n_tiles * (long long)kTileP;
     const long long need = (total + 255) / 256, cap = 8LL * num_sms();
-    k_blocked_dense<<<(int)(need < cap ? need : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(total, n_tokens, b->lid, b->tok, hcoef, H);
+    k_blocked_dense<<<(int)(need < cap ? need : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(total, n_tokens, b->pw, b->tok, hcoef, H);
     return check_launch();
 }
 

@@ -6,11 +6,14 @@
 // The sparsity pattern (local_indices, arbitrage.py:6-12) is static across dual iterations, so it is preprocessed once
 // into tiles of P pools whose tokens fall in two narrow token blocks:
 //   * a tile touches few distinct tokens: nu is gathered once per tile into shared memory (nu_local) and the pools
-//     address it with 16-bit local ids (4 B/pool instead of 8 B of global indices);
-//   * each pool thread writes its two net flows to a shared-memory array g[2P] in ROW order (no atomics);
+//     address it with 10-bit local ids;
+//   * each pool thread writes its two net flows to a shared-memory array g[2P] (no atomics): slot 0 to g[l] (pool
+//     order: the pools of a tile are sorted by slot-0 token, so a token's slot-0 flows are already neighbours), slot 1 to
+//     g[P + p1], where p1 is the pool's rank among the tile's slot-1 half-edges stably sorted by token;
 //   * "rows" = (token, <=32 consecutive entries of g) listed by a per-tile table are summed by one thread each, in a
 //     fixed order (bit-reproducible), and only the row totals go to global memory: ~0.36 red.add per pool instead of 2.
-// HBM bytes per pool: 3 x 8 (R0, R1, 1/gamma) + 4 (local ids) + 4 (row positions) + ~1-2 (row/token tables).
+// One 32-bit word per pool carries both local ids and p1 (lid0 | lid1 << 10 | p1 << 20).
+// HBM bytes per pool: 3 x 8 (R0, R1, 1/gamma) + 4 (pool word) + ~3 (row/token tables).
 // Pool slabs and the per-tile tables are staged through a shared-memory ring by 1-D bulk TMA copies
 // (cp.async.bulk + mbarrier).
 #pragma once
@@ -32,23 +35,28 @@ constexpr int kTileP = CFMM_TILE_P;  // pools per tile: 1M pools = 977 tiles ove
 constexpr int kTileT = kTileP / 2;   // threads per CTA: two pools per thread
 constexpr int kTileStages = 2;       // TMA ring depth
 constexpr int kCtasPerSm = CFMM_CTAS_PER_SM;
-static_assert(kTileP % 64 == 0 && kTileP <= 1024, "tile size: whole warps of two-pool threads, 10-bit local token ids");
+static_assert(kTileP % 64 == 0 && kTileP <= 1024, "tile size: whole warps of two-pool threads, 10-bit fields of the pool word");
+
+// pool word: local token id of slot 0 (10 bits) | of slot 1 (10 bits) << 10 | p1 (10 bits) << 20, where p1 = position of
+// the slot-1 flow in the second half of the tile's flow array g (the slot-0 flow of pool l goes to g[l])
+__device__ __forceinline__ int pw_lid0(uint32_t w) { return (int)(w & 0x3ffu); }
+__device__ __forceinline__ int pw_lid1(uint32_t w) { return (int)((w >> 10) & 0x3ffu); }
+__device__ __forceinline__ int pw_pos1(uint32_t w) { return (int)(w >> 20); }
 
 template <int P>
 struct BlockedCfg {
-    // the layout builder guarantees <= P distinct tokens per tile (tiles that would exceed it go to the
-    // plain bucket), so rows <= P + 2P/32 (every token one row, plus one extra row per 32 entries)
+    // the layout builder guarantees <= P distinct tokens and <= kRowsMax rows per tile (tiles that would exceed
+    // either go to the plain bucket)
     static constexpr int kTokMax = P;
     static constexpr int kRowCapMin = 8;                     // smallest row cap the tables are sized for
     static constexpr int kRowsMax = P + 2 * P / kRowCapMin + 8;
 };
 
-// one ring stage: NF per-pool f64 slabs + local ids + row positions + row table + token list
+// one ring stage: NF per-pool f64 slabs + pool words + row table + token list
 template <int P, int NF>
 struct __align__(128) Stage {
     double a[NF][P];
-    uint32_t lid[P];                              // lid0 | lid1 << 16
-    uint32_t pos[P];                              // where this pool's two flows go in the row-ordered array g: pos0 | pos1 << 16
+    uint32_t pw[P];                               // lid0 | lid1 << 10 | p1 << 20
     uint32_t rows[BlockedCfg<P>::kRowsMax];       // start :16 | length (1..32) :6 | local token :10, longest first
     int32_t tok[BlockedCfg<P>::kTokMax];          // local token id -> global token id
     int4 desc;                                    // (ntok, nrow, 0, 0) of the tile in this stage
@@ -58,8 +66,7 @@ struct BlockedArgs {
     long long n_tiles;
     long long M;                  // n_tiles * P (padded pool count = slab stride)
     const double* slab[3];        // NF slabs, each [M]
-    const uint32_t* lid;          // [M]
-    const uint32_t* pos;          // [M]
+    const uint32_t* pw;           // [M] pool words
     const uint32_t* rows;         // [n_tiles][kRowsMax]
     const int32_t* tok;           // [n_tiles][kTokMax]
     const int4* desc;             // [n_tiles] (ntok, nrow, 0, 0)
@@ -83,12 +90,11 @@ __device__ __forceinline__ void issue_tile(Stage<P, NF>* st, uint64_t* bar, cons
     const unsigned rows_b = round16(4u * (unsigned)d.y);
     const unsigned tok_b = round16(4u * (unsigned)d.x);
     const long long off = tile * P;
-    mbar_expect_tx(bar, (unsigned)(NF * P * 8 + P * 4 + P * 4 + 16) + rows_b + tok_b);
+    mbar_expect_tx(bar, (unsigned)(NF * P * 8 + P * 4 + 16) + rows_b + tok_b);
     bulk_g2s(&st->desc, A.desc + tile, 16, bar);
 #pragma unroll
     for (int k = 0; k < NF; ++k) bulk_g2s(st->a[k], A.slab[k] + off, P * 8, bar);
-    bulk_g2s(st->lid, A.lid + off, P * 4, bar);
-    bulk_g2s(st->pos, A.pos + off, P * 4, bar);
+    bulk_g2s(st->pw, A.pw + off, P * 4, bar);
     bulk_g2s(st->rows, A.rows + tile * BlockedCfg<P>::kRowsMax, rows_b, bar);
     bulk_g2s(st->tok, A.tok + tile * BlockedCfg<P>::kTokMax, tok_b, bar);
 }
@@ -149,7 +155,7 @@ __device__ __forceinline__ double gather_vec(const BlockedArgs& A, int t) {
     return load_vec<COHERENT>(A.vec + t);
 }
 
-// Shared memory of one CTA of the TMA-staged pass: STAGES ring stages, nu_local [P], flows in row order [2P]
+// Shared memory of one CTA of the TMA-staged pass: STAGES ring stages, nu_local [P], flows [2P]
 template <int P, int STAGES>
 constexpr size_t pass_smem_bytes(int nf) {
     return (size_t)STAGES * (nf == 3 ? sizeof(Stage<P, 3>) : sizeof(Stage<P, 1>)) + (size_t)(3 * P) * sizeof(double);
@@ -167,7 +173,7 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
     using St = Stage<P, NF>;
     St* stages = reinterpret_cast<St*>(smem_raw);
     double* nul = reinterpret_cast<double*>(smem_raw + (size_t)STAGES * sizeof(St));      // [P]    nu_local
-    double* g = nul + P;                                                                   // [2P] flows in ROW order
+    double* g = nul + P;                                                                   // [2P] flows: slot 0 | slot 1
     const int tid = threadIdx.x;
     // Each CTA walks a CONTIGUOUS chunk of tiles.  Tiles are sorted by (token block of slot 0, of slot 1), so at any
     // moment the resident CTAs work on different token blocks and their red.adds hit different addresses (a
@@ -206,22 +212,22 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
         const long long far = tile + STAGES;
         int4 dfar = make_int4(0, 0, 0, 0);
         if (tid == 0 && far < t_end) dfar = __ldg(A.desc + far);
-        // ---- pool phase: per-pool flows, scattered into row order.  All loads and math of the thread's NPOOL pools
-        // first, the shared-memory stores afterwards, so the independent chains overlap in the pipeline.
+        // ---- pool phase: per-pool flows, slot 0 to g[l], slot 1 to g[P + p1].  All loads and math of the thread's NPOOL
+        // pools first, the shared-memory stores afterwards, so the independent chains overlap in the pipeline.
         {
             constexpr int NPOOL = P / THREADS;
             double f0[NPOOL], f1[NPOOL];
-            uint32_t ps[NPOOL];
+            uint32_t ws[NPOOL];
 #pragma unroll
             for (int u = 0; u < NPOOL; ++u) {
                 const int l = tid + u * THREADS;
-                const uint32_t li = S.lid[l];
-                ps[u] = S.pos[l];
+                const uint32_t w = S.pw[l];
+                ws[u] = w;
                 if (MODE == 0) {
                     EvalOp::apply<TRADES, HESS>(A, tile * P + l, S.a[0][l], S.a[NF > 1 ? 1 : 0][l], S.a[NF > 2 ? 2 : 0][l],
-                                                nul[li & 0xffffu], nul[li >> 16], f0[u], f1[u], acc);
+                                                nul[pw_lid0(w)], nul[pw_lid1(w)], f0[u], f1[u], acc);
                 } else if (MODE == 1) {
-                    const double pa = nul[li & 0xffffu], pb = nul[li >> 16], h = S.a[0][l];
+                    const double pa = nul[pw_lid0(w)], pb = nul[pw_lid1(w)], h = S.a[0][l];
                     f0[u] = h * (pa - pb);
                     f1[u] = -f0[u];
                     if (COHERENT) {                    // the persistent solver's PCG: p'Hp and p'diag(H)p come with the pass
@@ -235,8 +241,8 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
             }
 #pragma unroll
             for (int u = 0; u < NPOOL; ++u) {
-                g[ps[u] & 0xffffu] = f0[u];
-                g[ps[u] >> 16] = f1[u];
+                g[tid + u * THREADS] = f0[u];
+                g[P + pw_pos1(ws[u])] = f1[u];
             }
         }
         __syncthreads();                 // g complete; nu_local of this tile is dead from here on
@@ -256,8 +262,8 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
                 }
             }
         }
-        // ---- row phase: one thread per row; a row is a CONTIGUOUS run of g (the pool phase scattered the flows
-        // into row order), rows are sorted by length so a warp's 32 rows have (nearly) equal trip counts.
+        // ---- row phase: one thread per row; a row is a CONTIGUOUS run of g (flows of one token in one half), rows
+        // are sorted by length so a warp's 32 rows have (nearly) equal trip counts.
         // Fixed summation order; one red.add per row.
         for (int r = tid; r < d.y; r += THREADS) {
             const uint32_t rw = S.rows[r];

@@ -7,9 +7,10 @@
 //                       tokens fall into the same pair of narrow token blocks become neighbours; also validates the data
 //   2. cub radix sort   of (key, pool id) pairs: the blocked order
 //   3. k_build_tiles    ONE CTA PER TILE, everything in shared memory: sort the tile's 2P half-edges by token, number
-//                       the distinct tokens (16-bit local ids, token list), cut every token's run of flows into rows of
-//                       <= row_cap entries, order the rows longest first, give every half-edge its slot in the
-//                       row-ordered flow array, and gather the reserves / 1/gamma slabs into blocked order.
+//                       the distinct tokens (local ids, token list), rank the slot-1 half-edges in token order (their
+//                       positions in the flow array), cut the runs of equal tokens in both halves of the flow array
+//                       into rows of <= row_cap entries, order the rows longest first, and gather the reserves /
+//                       1/gamma slabs into blocked order.
 // It replaces ~240 torch launches (sort / unique / bincount / repeat_interleave / index ...) and their host round trips.
 #include <cub/cub.cuh>
 
@@ -34,11 +35,16 @@ struct BuildArgs {
     const double* gamma;       // [m]
     const uint32_t* order;     // [m] sorted pool ids (blocked position -> pool)
     double *r0, *r1, *gi;      // [T * P]
-    uint32_t *lid, *pos;       // [T * P]
+    uint32_t* pw;              // [T * P]
     uint32_t* rows;            // [T][LR]
     int32_t* tok;              // [T][P]
     int4* desc;                // [T]
-    int32_t* status;           // [0] tiles touching more than P tokens, [1] invalid pools, [2] total rows
+    int32_t* status;           // [0] tiles touching more than P tokens or needing more than LR rows, [1] invalid pools,
+                               // [2] total rows
+};
+
+struct MaxOp {
+    __device__ __forceinline__ int operator()(int a, int b) const { return a > b ? a : b; }
 };
 
 __global__ void __launch_bounds__(256)
@@ -63,32 +69,38 @@ using Scan = cub::BlockScan<int, LT>;
 
 struct TileSmem {                          // dynamic shared memory of one tile CTA (> 48 KB with the cub scratch)
     union { typename Sort::TempStorage sort; typename Scan::TempStorage scan; } tmp;
-    uint32_t sk[LH];                       // half-edges sorted by token: token id; later: row sort keys / sorted row lengths
+    uint32_t sk[LH];                       // half-edges sorted by token: token id
     uint32_t sv[LH];                       //                              slot << 15 | pool-in-tile
     uint16_t gid[LH];                      // local token id of every sorted half-edge
-    int gs[LP + 2];                        // first sorted half-edge of every local token (+ end)
-    int rfirst[LP + 1];                    // first row of every local token
-    uint16_t rrank[LR + 8];                // old row id -> position after the longest-first sort
-    int rstart[LR + 8];                    // sorted position -> first slot of the row in the flow array
-    uint16_t lidh[LP][2], posh[LP][2];
-    int ntok, nrow;
+    uint16_t ftok[LH];                     // local token of the flow at every position of the flow array (slot 0 | slot 1)
+    uint16_t rlen[LH];                     // length of the run of equal tokens that starts at a position of the flow array
+    uint16_t lidh[LP][2], p1h[LP];         // local ids and slot-1 position of every pool
+    int ntok;
 };
+
+// a tile the layout cannot hold: counted in status[0], its slabs and tables kept inert (never launched: the host falls back)
+__device__ void inert_tile(const BuildArgs& B, long long tile) {
+    const long long p0 = tile * LP;
+    if (threadIdx.x == 0) { atomicAdd(B.status, 1); B.desc[tile] = make_int4(0, 0, 0, 0); }
+    for (int l = threadIdx.x; l < LP; l += LT) {
+        B.r0[p0 + l] = 1.0; B.r1[p0 + l] = 1.0; B.gi[p0 + l] = 1.0; B.pw[p0 + l] = 0u;
+    }
+}
 
 __global__ void __launch_bounds__(LT)
 k_build_tiles(const BuildArgs B) {
     extern __shared__ __align__(16) unsigned char tile_smem_raw[];
     TileSmem& M = *reinterpret_cast<TileSmem*>(tile_smem_raw);
     auto& tmp = M.tmp;
-    uint32_t* sk = M.sk; uint32_t* sv = M.sv; uint16_t* gid = M.gid; int* gs = M.gs; int* rfirst = M.rfirst;
-    uint32_t* rk = M.sk;                   // the token ids are dead once the token list is written
-    uint16_t* rrank = M.rrank; int* rstart = M.rstart;
-    auto& lidh = M.lidh; auto& posh = M.posh;
-    int& s_ntok = M.ntok; int& s_nrow = M.nrow;
+    uint32_t* sk = M.sk; uint32_t* sv = M.sv; uint16_t* gid = M.gid; uint16_t* ftok = M.ftok; uint16_t* rlen = M.rlen;
+    auto& lidh = M.lidh; uint16_t* p1h = M.p1h;
+    int& s_ntok = M.ntok;
     const int tid = threadIdx.x;
     const long long tile = blockIdx.x;
     const long long p0 = tile * LP;
     const int np = (int)(B.m - p0 < LP ? B.m - p0 : LP);               // real pools in this tile
     const int nh = 2 * np;
+    auto real = [&](int c) { return (c < LP ? c : c - LP) < np; };     // position c of the flow array holds a real flow
     // ---- 1. the tile's half-edges, slot-major (slot 0 of every pool, then slot 1), sorted by token (stable)
     uint32_t key[LI], val[LI];
 #pragma unroll
@@ -107,7 +119,7 @@ k_build_tiles(const BuildArgs B) {
 #pragma unroll
     for (int u = 0; u < LI; ++u) { sk[tid * LI + u] = key[u]; sv[tid * LI + u] = val[u]; }
     __syncthreads();
-    // ---- 2. distinct tokens: heads -> local ids (exclusive scan), token list, group starts
+    // ---- 2. distinct tokens: heads -> local ids (exclusive scan), token list
     int head[LI], gpre[LI];
 #pragma unroll
     for (int u = 0; u < LI; ++u) {
@@ -117,105 +129,92 @@ k_build_tiles(const BuildArgs B) {
     int ntok;
     Scan(tmp.scan).ExclusiveSum(head, gpre, ntok);
     __syncthreads();
-    const bool bad = ntok > LP;                                          // more tokens than a tile may touch: not blockable
+    if (ntok > LP) { inert_tile(B, tile); return; }                      // more tokens than a tile may touch: not blockable
 #pragma unroll
     for (int u = 0; u < LI; ++u) {
         const int i = tid * LI + u;
         if (i < nh) {
             const int g = gpre[u] + head[u] - 1;                         // local id of this half-edge's token
             gid[i] = (uint16_t)g;
-            if (head[u] && !bad) { gs[g] = i; B.tok[tile * LP + g] = (int32_t)sk[i]; }
+            if (head[u]) B.tok[tile * LP + g] = (int32_t)sk[i];
         }
     }
-    if (tid == 0) { s_ntok = ntok; if (!bad) gs[ntok] = nh; }
+    if (tid == 0) s_ntok = ntok;
     __syncthreads();
-    if (bad) {
-        if (tid == 0) { atomicAdd(B.status, 1); B.desc[tile] = make_int4(0, 0, 0, 0); }
-        // keep the slabs and tables inert: unit reserves, zero ids / positions (never launched: the host falls back)
-        for (int l = tid; l < LP; l += LT) {
-            B.r0[p0 + l] = 1.0; B.r1[p0 + l] = 1.0; B.gi[p0 + l] = 1.0; B.lid[p0 + l] = 0u; B.pos[p0 + l] = 0u;
-        }
-        return;
+    // ---- 3. local ids of every pool; a slot-1 half-edge's rank among the slot-1 half-edges in token order (stable: pool
+    // order within a token) is the position of its flow in the second half of the flow array, a slot-0 flow sits at its pool
+    int s1[LI], p1[LI];
+#pragma unroll
+    for (int u = 0; u < LI; ++u) {
+        const int i = tid * LI + u;
+        s1[u] = (i < nh && (sv[i] >> 15)) ? 1 : 0;
     }
-    // ---- 3. rows: every token's run of flows is cut into rows of <= row_cap entries
+    Scan(tmp.scan).ExclusiveSum(s1, p1);
+#pragma unroll
+    for (int u = 0; u < LI; ++u) {
+        const int i = tid * LI + u;
+        if (i < nh) {
+            const uint32_t v = sv[i];
+            const int slot = v >> 15, l = v & 0x7fffu;
+            lidh[l][slot] = gid[i];
+            if (slot) { p1h[l] = (uint16_t)p1[u]; ftok[LP + p1[u]] = gid[i]; }
+            else ftok[l] = gid[i];
+        }
+    }
+    __syncthreads();
+    // ---- 4. runs of equal tokens in each half of the flow array: slot 0 in pool order (the pools are sorted by slot-0
+    // token within a key block), slot 1 in token order.  Every position learns where its run starts; run ends record
+    // the run's length at the start
+    int hs[LI], rs[LI];
+#pragma unroll
+    for (int u = 0; u < LI; ++u) {
+        const int c = tid * LI + u;
+        hs[u] = (real(c) && (c == 0 || c == LP || ftok[c] != ftok[c - 1])) ? c : -1;
+    }
+    Scan(tmp.scan).InclusiveScan(hs, rs, MaxOp());
+#pragma unroll
+    for (int u = 0; u < LI; ++u) {
+        const int c = tid * LI + u;
+        if (real(c) && (c + 1 == LP || c + 1 == LH || !real(c + 1) || ftok[c + 1] != ftok[c])) rlen[rs[u]] = (uint16_t)(c - rs[u] + 1);
+    }
+    __syncthreads();
+    // ---- 5. rows: every run cut into rows of <= row_cap entries, sorted longest first (the 32 rows a warp sums then
+    // have nearly equal trip counts; ties in flow-array order).  Key: (63 - length) << 11 | start
     const int cap = B.row_cap;
-    int nsub[2], rpre[2];                                                 // LT * 2 = LP >= ntok tokens
+    uint32_t rkey[LI], rdum[LI];
+    int nrow = 0;
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
-        const int g = tid * 2 + u;
-        nsub[u] = g < ntok ? (gs[g + 1] - gs[g] + cap - 1) / cap : 0;
+    for (int u = 0; u < LI; ++u) {
+        const int c = tid * LI + u;
+        const int o = c - rs[u];
+        const bool rh = real(c) && o % cap == 0;
+        rkey[u] = rh ? (uint32_t)(63 - min(cap, (int)rlen[rs[u]] - o)) << 11 | (uint32_t)c : 0xffffffffu;
+        rdum[u] = 0u;
+        nrow += __syncthreads_count(rh);
     }
-    int nrow;
-    Scan(tmp.scan).ExclusiveSum(nsub, rpre, nrow);
-    __syncthreads();
+    if (nrow > LR) { inert_tile(B, tile); return; }                      // more rows than the row table holds: not blockable
+    Sort(tmp.sort).Sort(rkey, rdum, 0, 17);
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
-        const int g = tid * 2 + u;
-        if (g < ntok) {
-            rfirst[g] = rpre[u];
-            const int cnt = gs[g + 1] - gs[g];
-            for (int s = 0; s < nsub[u]; ++s) {                          // old row id rpre + s: (63 - len) << 16 | id, ltok kept aside
-                const int len = min(cap, cnt - cap * s);
-                rk[rpre[u] + s] = (uint32_t)(63 - len) << 16 | (uint32_t)(rpre[u] + s);
-            }
+    for (int u = 0; u < LI; ++u) {
+        const int r = tid * LI + u;
+        if (r < nrow) {
+            const int c = (int)(rkey[u] & 0x7ffu);
+            B.rows[tile * LR + r] = (uint32_t)c | (uint32_t)(63 - (int)(rkey[u] >> 11)) << 16 | (uint32_t)ftok[c] << 22;
         }
     }
-    if (tid == 0) s_nrow = nrow;
-    __syncthreads();
-    // ---- 4. longest rows first (the 32 rows a warp sums then have nearly equal trip counts): sort the row keys
-    uint32_t rkey[LI], rdum[LI];
-#pragma unroll
-    for (int u = 0; u < LI; ++u) {
-        const int r = tid * LI + u;
-        rkey[u] = r < nrow ? rk[r] : 0xffffffffu;
-        rdum[u] = 0u;
-    }
-    __syncthreads();
-    Sort(tmp.sort).Sort(rkey, rdum, 0, 22);
-    int rlen[LI], spre[LI];
-#pragma unroll
-    for (int u = 0; u < LI; ++u) {
-        const int r = tid * LI + u;
-        rlen[u] = r < nrow ? 63 - (int)(rkey[u] >> 16) : 0;
-        if (r < nrow) rrank[rkey[u] & 0xffffu] = (uint16_t)r;
-    }
-    __syncthreads();
-    int total;
-    Scan(tmp.scan).ExclusiveSum(rlen, spre, total);
-#pragma unroll
-    for (int u = 0; u < LI; ++u) {
-        const int r = tid * LI + u;
-        if (r < nrow) { rstart[r] = spre[u]; rk[r] = (uint32_t)rlen[u]; }          // rk now: length of sorted row r
-    }
-    __syncthreads();
-    // ---- 5. every half-edge: its row, its slot in the row-ordered flow array; the row table
-    for (int i = tid; i < nh; i += LT) {
-        const int g = gid[i], o = i - gs[g];
-        const int r = rrank[rfirst[g] + o / cap];
-        const int p = rstart[r] + o % cap;
-        const uint32_t v = sv[i];
-        const int slot = v >> 15, l = v & 0x7fffu;
-        lidh[l][slot] = (uint16_t)g;
-        posh[l][slot] = (uint16_t)p;
-        if (o % cap == 0) B.rows[tile * LR + r] = (uint32_t)rstart[r] | rk[r] << 16 | (uint32_t)g << 22;
-    }
-    __syncthreads();
-    // ---- 6. per-pool words and slabs, blocked order; padding pools write zero flows past the real entries
+    // ---- 6. pool words and slabs, blocked order; padding pool l writes zero flows to g[l] and g[P + l], past the real ones
     for (int l = tid; l < LP; l += LT) {
         if (l < np) {
             const uint32_t pool = B.order[p0 + l];
-            B.lid[p0 + l] = (uint32_t)lidh[l][0] | (uint32_t)lidh[l][1] << 16;
-            B.pos[p0 + l] = (uint32_t)posh[l][0] | (uint32_t)posh[l][1] << 16;
+            B.pw[p0 + l] = (uint32_t)lidh[l][0] | (uint32_t)lidh[l][1] << 10 | (uint32_t)p1h[l] << 20;
             B.r0[p0 + l] = B.R[2 * (long long)pool]; B.r1[p0 + l] = B.R[2 * (long long)pool + 1];
             B.gi[p0 + l] = 1.0 / B.gamma[pool];
         } else {
-            const int pl = l - np;
-            B.lid[p0 + l] = 0u;
-            B.pos[p0 + l] = (uint32_t)(nh + 2 * pl) | (uint32_t)(nh + 2 * pl + 1) << 16;
+            B.pw[p0 + l] = (uint32_t)l << 20;
             B.r0[p0 + l] = 1.0; B.r1[p0 + l] = 1.0; B.gi[p0 + l] = 1.0;
         }
     }
-    if (tid == 0) { B.desc[tile] = make_int4(s_ntok, s_nrow, 0, 0); atomicAdd(B.status + 2, s_nrow); }
+    if (tid == 0) { B.desc[tile] = make_int4(s_ntok, nrow, 0, 0); atomicAdd(B.status + 2, nrow); }
 }
 
 inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -239,9 +238,10 @@ int64_t cfmm_blocked_build_work_bytes(int64_t n_pools) {
 /* Build the token-blocked layout of m constant-product pools on the device.  idx [m][2] int32, reserves [m][2] f64,
  * gamma [m] f64: the reference's local_indices / reserves / fees (arbitrage.py:6-28) as contiguous device arrays.
  * `out`: a cfmm_blocked_pairs whose array members point at caller-allocated device buffers of n_tiles = ceil(m / P)
- * tiles (strides from cfmm_blocked_layout_info); r0 / r1 / gamma_inv / lid / pos / rows / tok / desc are filled.
+ * tiles (strides from cfmm_blocked_layout_info); r0 / r1 / gamma_inv / pw / rows / tok / desc are filled.
  * order [m] uint32 (device, out): pool at every blocked position.  status [4] int32 (device, zeroed by this call, out):
- * [0] tiles that touch more tokens than a tile may (the caller must fall back to a plain bucket for such problems),
+ * [0] tiles that touch more tokens, or need more rows, than a tile may (the caller must fall back to a plain bucket for
+ * such problems),
  * [1] CTAs that saw invalid pools (reserves <= 0 or not finite, fees outside (0, 1], token ids out of range or equal),
  * [2] total rows.  Asynchronous on `stream`. */
 int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, const double* reserves, const double* gamma,
@@ -252,7 +252,8 @@ int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, co
     if (work_bytes < cfmm_blocked_build_work_bytes(n_pools)) return CFMM_E_SIZE;
     const long long T = (n_pools + LP - 1) / LP;
     if (out->pools_per_tile != LP || out->n_tiles != T || out->n_pools != n_pools) return CFMM_E_SIZE;
-    if (!out->r0 || !out->r1 || !out->gamma_inv || !out->lid || !out->pos || !out->rows || !out->tok || !out->desc) return CFMM_E_NULL;
+    if (!out->r0 || !out->r1 || !out->gamma_inv || !out->pw || !out->rows || !out->tok || !out->desc) return CFMM_E_NULL;
+    if (out->reserved_ptr) return CFMM_E_KIND;
     int row_cap = 32;
     cfmm_blocked_layout_info(nullptr, nullptr, nullptr, &row_cap);
     long long nb = (long long)llround(sqrt((double)n_pools / LP));
@@ -282,7 +283,7 @@ int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, co
     B.m = n_pools; B.n_tokens = n_tokens; B.nb = (int)nb; B.row_cap = row_cap; B.key_bits = key_bits; B.tok_bits = 32;
     B.idx = idx; B.R = reserves; B.gamma = gamma; B.order = order;
     B.r0 = const_cast<double*>(out->r0); B.r1 = const_cast<double*>(out->r1); B.gi = const_cast<double*>(out->gamma_inv);
-    B.lid = const_cast<uint32_t*>(out->lid); B.pos = const_cast<uint32_t*>(out->pos);
+    B.pw = const_cast<uint32_t*>(out->pw);
     B.rows = const_cast<uint32_t*>(out->rows); B.tok = const_cast<int32_t*>(out->tok);
     B.desc = reinterpret_cast<int4*>(const_cast<int32_t*>(out->desc));
     B.status = status;

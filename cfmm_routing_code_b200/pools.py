@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+from collections.abc import Mapping
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -273,19 +274,101 @@ def blocked_layout_info(lib):
     return tuple(int(x.value) for x in v)      # pools_per_tile, rows_stride, tok_stride, row_cap
 
 
+def unpack_pool_words(pw: torch.Tensor, P: int):
+    """Pool words of a blocked layout (``lid0 | lid1 << 10 | p1 << 20``, see csrc/cfmm_blocked.cuh) in the two-word form,
+    int32 each: local ids ``lid0 | lid1 << 16`` and flow-array positions ``pos0 | pos1 << 16``, where pos0 = l (the pool's
+    index in its tile) and pos1 = P + p1."""
+    w = pw.to(torch.int64) & 0xffffffff
+    l = torch.arange(w.numel(), device=w.device) % P
+    lid = (w & 0x3ff) | (((w >> 10) & 0x3ff) << 16)
+    pos = l | ((P + (w >> 20)) << 16)
+    return lid.to(torch.int32), pos.to(torch.int32)
+
+
+class BlockedTables(Mapping):
+    """The tables of a blocked layout, read-only and dict-like.  Stores the pool words ``pw``; ``lid`` and ``pos`` (the
+    two-word form of unpack_pool_words) are computed on access."""
+    _DERIVED = ("lid", "pos")
+
+    def __init__(self, P: int, **tables):
+        self._P = P
+        self._t = tables
+
+    def __getitem__(self, k):
+        if k in self._DERIVED:
+            return unpack_pool_words(self._t["pw"], self._P)[self._DERIVED.index(k)]
+        return self._t[k]
+
+    def __iter__(self):
+        return iter(list(self._t) + list(self._DERIVED))
+
+    def __len__(self):
+        return len(self._t) + len(self._DERIVED)
+
+
+def _tile_layout(a: torch.Tensor, b: torch.Tensor, n_tokens: int, P: int, row_cap: int) -> dict:
+    """Tables of the pools with tokens (a, b), in blocked order, cut into tiles of P (csrc/cfmm_blocked.cuh): local ids
+    numbered in token order, slot-1 positions, token lists, rows; and (ntok, nrow) per tile, to be checked against the
+    table strides before anything is written at those strides."""
+    dev = a.device
+    i64 = dict(dtype=torch.int64, device=dev)
+    mm = a.numel()
+    ntiles = -(-mm // P)
+    q = torch.arange(mm, **i64)
+    tile = q // P
+    # distinct tokens of every tile -> local ids and token list
+    ck, perm = torch.sort(torch.cat([tile, tile]) * n_tokens + torch.cat([a, b]), stable=True)
+    uniq, inv = torch.unique_consecutive(ck, return_inverse=True)
+    u_tile = uniq // n_tokens
+    ntok = torch.bincount(u_tile, minlength=ntiles)
+    ltok_u = torch.arange(uniq.numel(), **i64) - (torch.cumsum(ntok, 0) - ntok)[u_tile]
+    he_ltok = torch.empty(2 * mm, **i64)
+    he_ltok[perm] = ltok_u[inv]
+    lid0, lid1 = he_ltok[:mm], he_ltok[mm:]
+    # slot 1: rank among the tile's slot-1 half-edges stably sorted by token (every tile but the last holds P pools)
+    s1 = torch.argsort(tile * n_tokens + b, stable=True)
+    p1 = torch.empty(mm, **i64)
+    p1[s1] = q - tile[s1] * P
+    # the flow array of every tile: slot 0 at g[l], slot 1 at g[P + p1]; F = local token of each flow, -1 where none
+    F = torch.full((ntiles, 2 * P), -1, **i64)
+    F[tile, q - tile * P] = lid0
+    F[tile, P + p1] = lid1
+    F = F.view(-1)
+    c = torch.arange(F.numel(), **i64)
+    real = F >= 0
+    # runs of equal tokens inside each half, cut into rows of <= row_cap flows
+    head = real & ((c % P == 0) | (F != torch.roll(F, 1)))
+    start = torch.cummax(torch.where(head, c, -1), 0).values
+    run = torch.cumsum(head.to(torch.int64), 0) - 1
+    run_len = torch.bincount(run[real])
+    o = c - start
+    rh = real & (o % row_cap == 0)
+    rc = c[rh]
+    row_len = torch.clamp(run_len[run[rh]] - o[rh], max=row_cap)
+    row_tile, row_start = rc // (2 * P), rc % (2 * P)
+    # longest rows first inside each tile (the 32 rows a warp sums have nearly equal trip counts), ties in flow order
+    srt = torch.argsort((row_tile * 64 + (63 - row_len)) * (2 * P) + row_start)
+    row_tile, row_start, row_len, row_ltok = row_tile[srt], row_start[srt], row_len[srt], F[rc][srt]
+    nrow = torch.bincount(row_tile, minlength=ntiles)
+    return dict(ntiles=ntiles, ntok=ntok, nrow=nrow, uniq=uniq, u_tile=u_tile, ltok_u=ltok_u, lid0=lid0, lid1=lid1, p1=p1,
+                row_tile=row_tile, row_start=row_start, row_len=row_len, row_ltok=row_ltok)
+
+
 def build_blocked_pairs(idx: torch.Tensor, n_tokens: int, P: int, rows_stride: int, tok_stride: int, row_cap: int):
     """Layout builder for cfmm_blocked_pairs (see csrc/cfmm_blocked.cuh).  idx: (2, m) int64 token ids on the
-    device.  Pools are sorted by (token block of slot 0, token block of slot 1) and cut into tiles of P; each
-    tile gets its distinct-token list, 16-bit local ids, and a CSR of rows (token, <= row_cap entries).
+    device.  Pools are sorted by (token block of slot 0, token block of slot 1, slot-0 token) and cut into tiles of P;
+    each tile gets its distinct-token list, one pool word per pool (10-bit local ids, slot-1 flow position), and a table
+    of rows (token, <= row_cap consecutive flows).
     Returns (order, residual, tables): `order` = bucket-local pool index at each blocked position, `residual` =
-    pools left out because their tile would touch more than tok_stride tokens (they go to a plain bucket)."""
+    pools left out because their tile would touch more than tok_stride tokens or need more than rows_stride rows (they
+    go to a plain bucket), `tables` = BlockedTables."""
     dev = idx.device
     m = idx.shape[1]
     i64 = dict(dtype=torch.int64, device=dev)
     nb = max(1, int(round((m / P) ** 0.5)))
     a, b = idx[0], idx[1]
     # primary: (token block of slot 0, token block of slot 1); secondary: slot-0 token, so that the lanes of a warp
-    # read the same nu_local entry (shared-memory broadcast) and scatter slot-0 flows to consecutive positions
+    # read the same nu_local entry (shared-memory broadcast) and a token's slot-0 flows are neighbours in the flow array
     key = ((a * nb // n_tokens) * nb + (b * nb // n_tokens)) * n_tokens + a
     order = torch.argsort(key, stable=True)
     residual = []
@@ -293,74 +376,35 @@ def build_blocked_pairs(idx: torch.Tensor, n_tokens: int, P: int, rows_stride: i
         mm = order.numel()
         if mm == 0:
             break
-        pos = torch.arange(mm, **i64)
-        ntiles = -(-mm // P)
-        tile = pos // P
-        he_tok = torch.cat([a[order], b[order]])
-        he_tile = torch.cat([tile, tile])
-        ck, perm = torch.sort(he_tile * n_tokens + he_tok, stable=True)
-        uniq, inv, counts = torch.unique_consecutive(ck, return_inverse=True, return_counts=True)
-        u_tile = uniq // n_tokens
-        ntok = torch.bincount(u_tile, minlength=ntiles)
-        bad = ntok > tok_stride
+        L = _tile_layout(a[order], b[order], n_tokens, P, row_cap)
+        bad = (L["ntok"] > tok_stride) | (L["nrow"] > rows_stride)
         if not bool(bad.any()):
             break
         if _pass == 3:                       # give up blocking: everything left goes to the plain bucket
             residual.append(order); order = order[:0]; mm = 0
             break
-        keep = ~bad[tile]
+        keep = ~bad[torch.arange(mm, **i64) // P]
         residual.append(order[~keep])
         order = order[keep]
     residual = torch.cat(residual) if residual else order[:0]
     if order.numel() == 0:
         return order, residual, None
-    U = uniq.numel()
-    tok_off = torch.cumsum(ntok, 0) - ntok
-    ltok_u = torch.arange(U, **i64) - tok_off[u_tile]
-    he_ltok = torch.empty(2 * mm, **i64)
-    he_ltok[perm] = ltok_u[inv]
+    ntiles, ntok, nrow = L["ntiles"], L["ntok"], L["nrow"]
     M = ntiles * P
-    lid = torch.zeros(M, dtype=torch.int32, device=dev)
-    lid[:mm] = (he_ltok[:mm] | (he_ltok[mm:] << 16)).to(torch.int32)
+    # pool words; padding pool l of the last tile writes its zero flows to g[l] and g[P + l], past the real ones
+    pw = (torch.arange(M, **i64) % P) << 20
+    pw[:mm] = L["lid0"] | (L["lid1"] << 10) | (L["p1"] << 20)
     tok = torch.zeros((ntiles, tok_stride), dtype=torch.int32, device=dev)
-    tok[u_tile, ltok_u] = (uniq - u_tile * n_tokens).to(torch.int32)
-    nsub = (counts + row_cap - 1) // row_cap
-    n_rows = int(nsub.sum())
-    first_row_u = torch.cumsum(nsub, 0) - nsub
-    row_u = torch.repeat_interleave(torch.arange(U, **i64), nsub)
-    sub = torch.arange(n_rows, **i64) - first_row_u[row_u]
-    g_start = torch.cumsum(counts, 0) - counts
-    row_tile0 = u_tile[row_u]
-    row_len0 = torch.clamp(counts[row_u] - row_cap * sub, max=row_cap)
-    # longest rows first inside each tile: the 32 rows a warp sums have (nearly) equal trip counts
-    srt = torch.argsort(row_tile0 * 64 + (63 - row_len0), stable=True)
-    rank = torch.empty_like(srt); rank[srt] = torch.arange(n_rows, **i64)     # old row id -> sorted position
-    row_tile, row_len, row_ltok = row_tile0[srt], row_len0[srt], ltok_u[row_u][srt]
-    nrow = torch.bincount(row_tile, minlength=ntiles)
-    row_first = torch.cumsum(nrow, 0) - nrow
-    r_local = torch.arange(n_rows, **i64) - row_first[row_tile]
-    if int(nrow.max()) > rows_stride:
-        raise _lib.CfmmError("blocked layout: row table overflow (library/builder mismatch)")
-    # g positions: rows are contiguous runs of the tile's row-ordered array, in sorted-row order
-    cs = torch.cumsum(row_len, 0) - row_len
-    row_start = cs - cs[row_first][row_tile]                                    # per tile
-    he_o = torch.arange(2 * mm, **i64) - g_start[inv]                           # offset inside its token group
-    he_row = rank[first_row_u[inv] + he_o // row_cap]                           # sorted row id of each half-edge
-    he_pos = torch.empty(2 * mm, **i64)
-    he_pos[perm] = row_start[he_row] + he_o % row_cap                           # back to (pool, slot) order
-    pos = torch.zeros(M, dtype=torch.int32, device=dev)
-    # padding pools (last tile) write their zero flows to slots past the real entries of that tile
-    pad_base = 2 * (mm - (ntiles - 1) * P)
-    if M > mm:
-        padl = torch.arange(M - mm, **i64)
-        pos[mm:] = ((pad_base + 2 * padl) | ((pad_base + 2 * padl + 1) << 16)).to(torch.int32)
-    pos[:mm] = (he_pos[:mm] | (he_pos[mm:] << 16)).to(torch.int32)
+    tok[L["u_tile"], L["ltok_u"]] = (L["uniq"] - L["u_tile"] * n_tokens).to(torch.int32)
+    row_tile = L["row_tile"]
+    n_rows = row_tile.numel()
+    r_local = torch.arange(n_rows, **i64) - (torch.cumsum(nrow, 0) - nrow)[row_tile]
     rows = torch.zeros((ntiles, rows_stride), dtype=torch.int32, device=dev)
-    word = row_start | (row_len << 16) | (row_ltok << 22)          # start:16 | len:6 | ltok:10 (may set bit 31)
+    word = L["row_start"] | (L["row_len"] << 16) | (L["row_ltok"] << 22)          # start:16 | len:6 | ltok:10 (may set bit 31)
     rows[row_tile, r_local] = torch.where(word >= 2 ** 31, word - 2 ** 32, word).to(torch.int32)
     desc = torch.stack([ntok, nrow, torch.zeros_like(ntok), torch.zeros_like(ntok)], 1).to(torch.int32).contiguous()
-    tables = dict(n_tiles=ntiles, M=M, lid=lid, tok=tok, pos=pos, rows=rows, desc=desc,
-                  rows_per_pool=n_rows / mm, tok_per_tile=float(ntok.double().mean()))
+    tables = BlockedTables(P, n_tiles=ntiles, M=M, pw=pw.to(torch.int32), tok=tok, rows=rows, desc=desc,
+                           rows_per_pool=n_rows / mm, tok_per_tile=float(ntok.double().mean()))
     return order, residual, tables
 
 
@@ -413,7 +457,7 @@ class BlockedBucket:
         self.r1 = slab(R[order, 1], 1.0)
         self.gamma_inv = slab(1.0 / gam[order], 1.0)
         self.c_blocked = _lib.BlockedPairs(self.m, t["n_tiles"], P, 0, self.r0.data_ptr(), self.r1.data_ptr(),
-                                           self.gamma_inv.data_ptr(), t["lid"].data_ptr(), t["pos"].data_ptr(),
+                                           self.gamma_inv.data_ptr(), t["pw"].data_ptr(), None,
                                            t["rows"].data_ptr(), t["tok"].data_ptr(), t["desc"].data_ptr())
 
     def _build_native(self, hp, spec, device, lib, P, rows_stride, tok_stride) -> bool:
@@ -435,7 +479,7 @@ class BlockedBucket:
         R = torch.from_numpy(hp.reserves[2 * lo:2 * hi]).to(device, non_blocking=True)
         gam = torch.from_numpy(hp.gamma[lo:hi]).to(device, non_blocking=True)
         slabs = torch.empty((3, M), **f64)
-        words = torch.empty((2, M), **i32)
+        pw = torch.empty(M, **i32)
         rows = torch.empty((T, rows_stride), **i32)
         tok = torch.empty((T, tok_stride), **i32)
         desc = torch.empty((T, 4), **i32)
@@ -445,8 +489,8 @@ class BlockedBucket:
         if nbytes <= 0:
             return False
         work = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        cb = _lib.BlockedPairs(m, T, P, 0, slabs[0].data_ptr(), slabs[1].data_ptr(), slabs[2].data_ptr(), words[0].data_ptr(),
-                               words[1].data_ptr(), rows.data_ptr(), tok.data_ptr(), desc.data_ptr())
+        cb = _lib.BlockedPairs(m, T, P, 0, slabs[0].data_ptr(), slabs[1].data_ptr(), slabs[2].data_ptr(), pw.data_ptr(),
+                               None, rows.data_ptr(), tok.data_ptr(), desc.data_ptr())
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         rc = lib.cfmm_blocked_build(m, hp.n_tokens, idx.data_ptr(), R.data_ptr(), gam.data_ptr(), C.byref(cb), order.data_ptr(),
                                     status.data_ptr(), work.data_ptr(), nbytes, st)
@@ -456,7 +500,8 @@ class BlockedBucket:
         st_h = status.cpu()                       # the one synchronisation of the build
         if int(st_h[1]) != 0:
             raise ValueError("invalid pool data (reserves > 0 and finite, fees in (0, 1], two distinct token ids in range)")
-        if int(st_h[0]) != 0:                     # a tile touches more tokens than it may: general builder + plain residual bucket
+        if int(st_h[0]) != 0:                     # a tile touches more tokens / needs more rows than it may: general builder
+                                                  # + plain residual bucket
             return False
         self.order = order
         self.residual = np.zeros(0, np.int64)
@@ -464,8 +509,8 @@ class BlockedBucket:
         self.stride = M
         self.r0, self.r1, self.gamma_inv = slabs[0], slabs[1], slabs[2]
         self._keep = (idx, R, gam, work)          # the build is asynchronous: its inputs live as long as the bucket
-        self.tables = dict(n_tiles=T, M=M, lid=words[0], pos=words[1], rows=rows, tok=tok, desc=desc,
-                           rows_per_pool=int(st_h[2]) / m, tok_per_tile=None)
+        self.tables = BlockedTables(P, n_tiles=T, M=M, pw=pw, tok=tok, rows=rows, desc=desc,
+                                    rows_per_pool=int(st_h[2]) / m, tok_per_tile=None)
         self.c_blocked = cb
         return True
 
@@ -485,7 +530,7 @@ class BlockedBucket:
     def bytes_resident(self) -> int:
         if self.tables is None:
             return 0
-        ts = [self.r0, self.r1, self.gamma_inv] + [self.tables[k] for k in ("lid", "tok", "pos", "rows", "desc")]
+        ts = [self.r0, self.r1, self.gamma_inv] + [self.tables[k] for k in ("pw", "tok", "rows", "desc")]
         return sum(x.numel() * x.element_size() for x in ts)
 
     def out_struct(self, trades: bool, hess: bool):

@@ -95,9 +95,11 @@ int cfmm_hess_dense(const cfmm_bucket* bucket, int32_t n_tokens, const double* h
 /*
  * Token-blocked storage for constant-product pools (the HBM-bound kind).  Built once per problem from
  * local_indices (arbitrage.py:6-12) by the layout builder (pools.py: build_blocked_pairs); pools are
- * reordered into tiles of `pools_per_tile` whose tokens fall into two narrow token blocks.  Per pool 28 B of
- * slabs + 4 B of local ids + 4 B of row positions; per tile a token list, a row table and (ntok, nrow).  See csrc/cfmm_blocked.cu.
+ * reordered into tiles of `pools_per_tile` whose tokens fall into two narrow token blocks.  Per pool 24 B of
+ * slabs + one 4 B pool word; per tile a token list, a row table and (ntok, nrow).  See csrc/cfmm_blocked.cuh.
  * Strides of the per-tile tables come from cfmm_blocked_layout_info().
+ * The evaluation writes the two flows of pool l of a tile to a per-tile array g[2P]: slot 0 to g[l], slot 1 to g[P + p1];
+ * a row sums a contiguous run of g.
  */
 typedef struct cfmm_blocked_pairs {
     int64_t n_pools;          /* real pools (<= n_tiles * pools_per_tile; the rest is padding)          */
@@ -107,9 +109,9 @@ typedef struct cfmm_blocked_pairs {
     const double* r0;         /* [n_tiles*P] reserves of slot 0, blocked order        arbitrage.py:14-20 */
     const double* r1;         /* [n_tiles*P] reserves of slot 1                                          */
     const double* gamma_inv;  /* [n_tiles*P] 1 / fees[i]                              arbitrage.py:22-28 */
-    const uint32_t* lid;      /* [n_tiles*P] tile-local token ids: slot0 | slot1 << 16                   */
-    const uint32_t* pos;      /* [n_tiles*P] where the pool's two flows go in the tile's row-ordered array:
-                                 pos(slot 0) | pos(slot 1) << 16, each < 2P                              */
+    const uint32_t* pw;       /* [n_tiles*P] pool word: tile-local token ids lid0 | lid1 << 10 | p1 << 20, each < P;
+                                 p1 = rank of the slot-1 half-edge among the tile's, stably sorted by token  */
+    const void* reserved_ptr; /* must be NULL                                                             */
     const uint32_t* rows;     /* [n_tiles][rows_stride] start :16 | length 1..32 :6 | local token :10, longest first */
     const int32_t* tok;       /* [n_tiles][tok_stride] local token id -> global token id                 */
     const int32_t* desc;      /* [n_tiles][4] (ntok, nrow, 0, 0)                                          */
@@ -126,9 +128,9 @@ int cfmm_set_blocked_config(int32_t cfg);
  * [m][2] f64, fees as gamma [m] f64 (arbitrage.py:6-28), contiguous on the device -- become the blocked layout in three
  * launches (pool keys + validation, radix sort, one CTA per tile).  `out`: a cfmm_blocked_pairs with n_pools = m,
  * n_tiles = ceil(m / P), pools_per_tile = P whose array members point at caller-allocated device buffers (strides from
- * cfmm_blocked_layout_info; slabs / lid / pos of n_tiles * P entries); all of them are filled.  order [m] uint32 (out):
- * the pool at every blocked position.  status [4] int32 (device, out): [0] tiles that touch more tokens than a tile may
- * (then the layout is unusable: use a plain bucket), [1] != 0: invalid pools (reserves <= 0 or not finite, fees outside
+ * cfmm_blocked_layout_info; slabs / pw of n_tiles * P entries); all of them are filled.  order [m] uint32 (out):
+ * the pool at every blocked position.  status [4] int32 (device, out): [0] tiles that touch more tokens, or need more
+ * rows, than a tile may (then the layout is unusable: use a plain bucket), [1] != 0: invalid pools (reserves <= 0 or not finite, fees outside
  * (0, 1], token ids out of range or equal), [2] rows in total.  CFMM_E_SIZE if the sort keys would not fit 32 bits
  * (token_blocks^2 * n_tokens >= 2^32).  work: cfmm_blocked_build_work_bytes(m) bytes.  Asynchronous on `stream`.
  */
