@@ -37,7 +37,7 @@ class BlockedPairs(C.Structure):
     _fields_ = [
         ("n_pools", C.c_int64), ("n_tiles", C.c_int64), ("pools_per_tile", C.c_int32), ("reserved", C.c_int32),
         ("r0", C.c_void_p), ("r1", C.c_void_p), ("gamma_inv", C.c_void_p), ("pw", C.c_void_p),
-        ("reserved_ptr", C.c_void_p), ("rows", C.c_void_p), ("tok", C.c_void_p), ("desc", C.c_void_p),
+        ("fee", C.c_void_p), ("rows", C.c_void_p), ("tok", C.c_void_p), ("desc", C.c_void_p),
     ]
 
 
@@ -110,6 +110,8 @@ def load(build_if_missing: bool = True):
     lib.cfmm_hess_dense.argtypes = [C.POINTER(Bucket), i32, vp, vp, vp, vp]
     lib.cfmm_blocked_layout_info.argtypes = [C.POINTER(i32)] * 4
     lib.cfmm_blocked_layout_info.restype = C.c_int
+    lib.cfmm_blocked_fee_words.argtypes = []
+    lib.cfmm_blocked_fee_words.restype = i32
     lib.cfmm_set_blocked_config.argtypes = [i32]
     lib.cfmm_set_blocked_config.restype = C.c_int
     lib.cfmm_blocked_build_work_bytes.argtypes = [i64]

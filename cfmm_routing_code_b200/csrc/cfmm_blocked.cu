@@ -301,12 +301,12 @@ int fill_blocked_args(const cfmm_blocked_pairs* b, BlockedArgs& A) {
     if (!b) return CFMM_E_NULL;
     if (b->pools_per_tile != kTileP) return CFMM_E_KIND;          // layout built for another library version
     if (b->n_tiles < 0 || b->n_pools < 0 || b->n_pools > b->n_tiles * (int64_t)kTileP) return CFMM_E_SIZE;
-    if (b->reserved_ptr) return CFMM_E_KIND;                       // a separate position array: layout of an older library
     if (b->n_tiles > 0 && (!b->pw || !b->rows || !b->tok || !b->desc)) return CFMM_E_NULL;
     A.n_tiles = b->n_tiles;
     A.M = b->n_tiles * (int64_t)kTileP;                            // slab stride (= where slot 1 of delta / lambda starts)
     A.pw = b->pw; A.rows = b->rows; A.tok = b->tok;
     A.desc = reinterpret_cast<const int4*>(b->desc);
+    A.fee = b->fee;
     A.zero_next = nullptr; A.n_zero = 0;
     A.slab[0] = A.slab[1] = A.slab[2] = nullptr;
     A.vec = nullptr; A.vec2 = nullptr; A.beta = 0.0;
@@ -325,6 +325,8 @@ int cfmm_blocked_layout_info(int32_t* pools_per_tile, int32_t* rows_stride, int3
     if (row_cap) *row_cap = g_row_cap;
     return CFMM_OK;
 }
+
+int32_t cfmm_blocked_fee_words(void) { return fee_words<kTileP>(); }
 
 int cfmm_set_blocked_config(int32_t cfg) {
     if (cfg >= 300) { const int c = cfg - 300; if (c < 8 || c > 32) return CFMM_E_KIND; g_row_cap = c; return CFMM_OK; }

@@ -13,7 +13,12 @@
 //   * "rows" = (token, <=32 consecutive entries of g) listed by a per-tile table are summed by one thread each, in a
 //     fixed order (bit-reproducible), and only the row totals go to global memory: ~0.36 red.add per pool instead of 2.
 // One 32-bit word per pool carries both local ids and p1 (lid0 | lid1 << 10 | p1 << 20).
-// HBM bytes per pool: 3 x 8 (R0, R1, 1/gamma) + 4 (pool word) + ~3 (row/token tables).
+// Fees come from a few tiers, so most tiles see at most 16 distinct 1/gamma values: such a tile carries them in a
+// per-tile fee record (table of the distinct values + a 4-bit code per pool, 656 B at P = 1024) and the evaluation
+// reads 1/gamma from the table instead of streaming the tile's 1/gamma slab.  Tiles with more distinct values stream
+// the slab.
+// HBM bytes per pool of the evaluation: 2 x 8 (R0, R1) + 4 (pool word) + ~3 (row/token tables) + 0.64 (fee record), plus
+// 8 (1/gamma) on tiles that stream the slab.
 // Pool slabs and the per-tile tables are staged through a shared-memory ring by 1-D bulk TMA copies
 // (cp.async.bulk + mbarrier).
 #pragma once
@@ -52,14 +57,25 @@ struct BlockedCfg {
     static constexpr int kRowsMax = P + 2 * P / kRowCapMin + 8;
 };
 
-// one ring stage: NF per-pool f64 slabs + pool words + row table + token list
+// fee record of a tile (include/cfmm_b200.h): header (nfee, 0, 0, 0) | table of kFeeMax f64 | codes, 4 bits per pool.
+// nfee == 0: the tile has more than kFeeMax distinct 1/gamma values and streams its slab.
+constexpr int kFeeMax = 16;
+constexpr int kFeeTab = 4;                         // word of the table
+constexpr int kFeeCode = kFeeTab + 2 * kFeeMax;    // word of the first code
+template <int P>
+__host__ __device__ constexpr int fee_words() { return kFeeCode + P / 8; }
+static_assert(fee_words<kTileP>() % 4 == 0, "fee record: whole 16-byte units (one bulk copy)");
+__device__ __forceinline__ unsigned fee_code(const uint32_t* codes, int l) { return (codes[l >> 3] >> (4 * (l & 7))) & 15u; }
+
+// one ring stage: NF per-pool f64 slabs + pool words + row table + token list + fee record (NF == 3)
 template <int P, int NF>
 struct __align__(128) Stage {
-    double a[NF][P];
+    double a[NF][P];                              // a[2] (1/gamma) is not filled on a coded tile
     uint32_t pw[P];                               // lid0 | lid1 << 10 | p1 << 20
     uint32_t rows[BlockedCfg<P>::kRowsMax];       // start :16 | length (1..32) :6 | local token :10, longest first
     int32_t tok[BlockedCfg<P>::kTokMax];          // local token id -> global token id
     int4 desc;                                    // (ntok, nrow, 0, 0) of the tile in this stage
+    uint32_t fee[fee_words<P>()];                 // fee record of the tile (evaluation with a fee record only)
 };
 
 struct BlockedArgs {
@@ -70,6 +86,7 @@ struct BlockedArgs {
     const uint32_t* rows;         // [n_tiles][kRowsMax]
     const int32_t* tok;           // [n_tiles][kTokMax]
     const int4* desc;             // [n_tiles] (ntok, nrow, 0, 0)
+    const uint32_t* fee;          // [n_tiles][fee_words] fee records, or null (every tile streams its 1/gamma slab)
     const double* vec;            // nu (eval) or vt (hvp); unused for diag
     const double* vec2;           // hvp inside the persistent solver: the direction is vec2 + beta * vec (PCG's p = z + beta p, formed on the fly)
     double beta;
@@ -84,19 +101,32 @@ struct BlockedArgs {
 
 __device__ __forceinline__ unsigned round16(unsigned bytes) { return (bytes + 15u) & ~15u; }
 
+// nfee of a tile's fee record (0 = no record or a tile that streams its 1/gamma slab); read by the producer thread
+template <int P, int NF>
+__device__ __forceinline__ unsigned tile_nfee(const BlockedArgs& A, long long tile) {
+    return (NF == 3 && A.fee) ? __ldg(A.fee + tile * fee_words<P>()) : 0u;
+}
+
+// d = the tile's descriptor, nfee = tile_nfee of the tile.  The bytes the barrier expects and the copies issued follow
+// from the same (nslab, rec): a mismatch would leave the barrier waiting forever.
 template <int P, int NF>
 __device__ __forceinline__ void issue_tile(Stage<P, NF>* st, uint64_t* bar, const BlockedArgs& A, long long tile,
-                                           const int4 d) {
+                                           const int4 d, const unsigned nfee) {
+    const bool rec = NF == 3 && A.fee != nullptr;                   // the fee record rides along
+    const int nslab = rec && nfee != 0 ? NF - 1 : NF;               // coded tile: its 1/gamma slab (the last) stays behind
+    const unsigned fee_b = rec ? 4u * fee_words<P>() : 0u;
     const unsigned rows_b = round16(4u * (unsigned)d.y);
     const unsigned tok_b = round16(4u * (unsigned)d.x);
     const long long off = tile * P;
-    mbar_expect_tx(bar, (unsigned)(NF * P * 8 + P * 4 + 16) + rows_b + tok_b);
+    mbar_expect_tx(bar, (unsigned)(nslab * P * 8 + P * 4 + 16) + rows_b + tok_b + fee_b);
     bulk_g2s(&st->desc, A.desc + tile, 16, bar);
 #pragma unroll
-    for (int k = 0; k < NF; ++k) bulk_g2s(st->a[k], A.slab[k] + off, P * 8, bar);
+    for (int k = 0; k < NF; ++k)
+        if (k < nslab) bulk_g2s(st->a[k], A.slab[k] + off, P * 8, bar);
     bulk_g2s(st->pw, A.pw + off, P * 4, bar);
     bulk_g2s(st->rows, A.rows + tile * BlockedCfg<P>::kRowsMax, rows_b, bar);
     bulk_g2s(st->tok, A.tok + tile * BlockedCfg<P>::kTokMax, tok_b, bar);
+    if (rec) bulk_g2s(st->fee, A.fee + tile * fee_words<P>(), fee_b, bar);
 }
 
 // ---- per-pool operator: the two net flows (f0, f1) of a constant-product pool (arbitrage.py:68-70) ----------
@@ -181,7 +211,7 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) {
             const long long t = t_beg + s;
-            if (t < t_end) issue_tile<P, NF>(&stages[s], &full[s], A, t, __ldg(A.desc + t));
+            if (t < t_end) issue_tile<P, NF>(&stages[s], &full[s], A, t, __ldg(A.desc + t), tile_nfee<P, NF>(A, t));
         }
     }
     if (PDL) {
@@ -211,10 +241,14 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
         // the producer thread fetches the descriptor of the tile it will issue at the end of this iteration
         const long long far = tile + STAGES;
         int4 dfar = make_int4(0, 0, 0, 0);
-        if (tid == 0 && far < t_end) dfar = __ldg(A.desc + far);
+        unsigned nfar = 0;
+        if (tid == 0 && far < t_end) { dfar = __ldg(A.desc + far); nfar = tile_nfee<P, NF>(A, far); }
         // ---- pool phase: per-pool flows, slot 0 to g[l], slot 1 to g[P + p1].  All loads and math of the thread's NPOOL
         // pools first, the shared-memory stores afterwards, so the independent chains overlap in the pipeline.
+        // 1/gamma: from the tile's fee table on a coded tile (the same bits as its slab entry), else from the slab.
         {
+            const bool coded = NF == 3 && A.fee != nullptr && S.fee[0] != 0u;        // uniform over the tile
+            const double* ftab = reinterpret_cast<const double*>(S.fee + kFeeTab);
             constexpr int NPOOL = P / THREADS;
             double f0[NPOOL], f1[NPOOL];
             uint32_t ws[NPOOL];
@@ -224,7 +258,8 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
                 const uint32_t w = S.pw[l];
                 ws[u] = w;
                 if (MODE == 0) {
-                    EvalOp::apply<TRADES, HESS>(A, tile * P + l, S.a[0][l], S.a[NF > 1 ? 1 : 0][l], S.a[NF > 2 ? 2 : 0][l],
+                    const double gi = coded ? ftab[fee_code(S.fee + kFeeCode, l)] : S.a[NF > 2 ? 2 : 0][l];
+                    EvalOp::apply<TRADES, HESS>(A, tile * P + l, S.a[0][l], S.a[NF > 1 ? 1 : 0][l], gi,
                                                 nul[pw_lid0(w)], nul[pw_lid1(w)], f0[u], f1[u], acc);
                 } else if (MODE == 1) {
                     const double pa = nul[pw_lid0(w)], pb = nul[pw_lid1(w)], h = S.a[0][l];
@@ -288,7 +323,7 @@ __device__ __forceinline__ void blocked_pass(const BlockedArgs& A, unsigned char
         __syncthreads();                 // stage and g are free again; nu_local of the next tile is in place
         if (tid == 0 && far < t_end) {
             fence_proxy_async();
-            issue_tile<P, NF>(&S, &full[stage], A, far, dfar);
+            issue_tile<P, NF>(&S, &full[stage], A, far, dfar, nfar);
         }
         stage = nstage;
     }

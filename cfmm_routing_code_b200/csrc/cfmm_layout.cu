@@ -9,8 +9,8 @@
 //   3. k_build_tiles    ONE CTA PER TILE, everything in shared memory: sort the tile's 2P half-edges by token, number
 //                       the distinct tokens (local ids, token list), rank the slot-1 half-edges in token order (their
 //                       positions in the flow array), cut the runs of equal tokens in both halves of the flow array
-//                       into rows of <= row_cap entries, order the rows longest first, and gather the reserves /
-//                       1/gamma slabs into blocked order.
+//                       into rows of <= row_cap entries, order the rows longest first, gather the reserves /
+//                       1/gamma slabs into blocked order, and code the tile's 1/gamma values (fee record).
 // It replaces ~240 torch launches (sort / unique / bincount / repeat_interleave / index ...) and their host round trips.
 #include <cub/cub.cuh>
 
@@ -26,6 +26,8 @@ constexpr int LH = 2 * kTileP;             // half-edges per tile
 constexpr int LI = 4;                      // items per thread of the block sorts (LT * LI == LH)
 static_assert(LT * LI == LH, "block sort shape");
 constexpr int LR = BlockedCfg<kTileP>::kRowsMax;
+constexpr int LU = LP / LT;                // pools per thread in step 6
+constexpr int LF = fee_words<kTileP>();    // words of a fee record
 
 struct BuildArgs {
     long long m;
@@ -39,6 +41,7 @@ struct BuildArgs {
     uint32_t* rows;            // [T][LR]
     int32_t* tok;              // [T][P]
     int4* desc;                // [T]
+    uint32_t* fee;             // [T][LF] fee records, or null
     int32_t* status;           // [0] tiles touching more than P tokens or needing more than LR rows, [1] invalid pools,
                                // [2] total rows
 };
@@ -76,6 +79,8 @@ struct TileSmem {                          // dynamic shared memory of one tile 
     uint16_t rlen[LH];                     // length of the run of equal tokens that starts at a position of the flow array
     uint16_t lidh[LP][2], p1h[LP];         // local ids and slot-1 position of every pool
     int ntok;
+    unsigned long long wmin[LT / 32];      // per-warp minima of a block min
+    unsigned long long ftab[kFeeMax];      // the tile's distinct 1/gamma bit patterns, ascending
 };
 
 // a tile the layout cannot hold: counted in status[0], its slabs and tables kept inert (never launched: the host falls back)
@@ -84,6 +89,62 @@ __device__ void inert_tile(const BuildArgs& B, long long tile) {
     if (threadIdx.x == 0) { atomicAdd(B.status, 1); B.desc[tile] = make_int4(0, 0, 0, 0); }
     for (int l = threadIdx.x; l < LP; l += LT) {
         B.r0[p0 + l] = 1.0; B.r1[p0 + l] = 1.0; B.gi[p0 + l] = 1.0; B.pw[p0 + l] = 0u;
+    }
+    if (B.fee)
+        for (int k = threadIdx.x; k < LF; k += LT) B.fee[tile * LF + k] = 0u;
+}
+
+// minimum over the tile CTA (every thread gets it)
+__device__ unsigned long long block_min(unsigned long long x, TileSmem& M) {
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long y = __shfl_xor_sync(0xffffffffu, x, o);
+        x = y < x ? y : x;
+    }
+    if ((threadIdx.x & 31) == 0) M.wmin[threadIdx.x >> 5] = x;
+    __syncthreads();
+    x = M.wmin[0];
+    for (int k = 1; k < LT / 32; ++k) x = M.wmin[k] < x ? M.wmin[k] : x;
+    __syncthreads();
+    return x;
+}
+
+// ---- 7. fee record (include/cfmm_b200.h) of a tile whose pool l = tid + u * LT has 1/gamma bit pattern gib[u], padding
+// included: the distinct patterns in ascending order, one block min over the patterns above the last one per value
+// (positive doubles order like their bit patterns), then a 4-bit index per pool.  More than kFeeMax values: all zero.
+__device__ void fee_record(const BuildArgs& B, TileSmem& M, long long tile, const unsigned long long (&gib)[LU]) {
+    const int tid = threadIdx.x;
+    uint32_t* rec = B.fee + tile * LF;
+    unsigned long long last = 0;
+    int nfee = 0;
+    bool over = false;
+    for (;;) {
+        unsigned long long c = ~0ull;                       // a NaN pattern: never a 1/gamma
+#pragma unroll
+        for (int u = 0; u < LU; ++u)
+            if ((nfee == 0 || gib[u] > last) && gib[u] < c) c = gib[u];
+        c = block_min(c, M);                                // (its barriers publish ftab[] written below)
+        if (c == ~0ull) break;
+        if (nfee == kFeeMax) { over = true; break; }
+        if (tid == 0) M.ftab[nfee] = c;
+        last = c;
+        ++nfee;
+    }
+    if (over) nfee = 0;
+    if (tid < kFeeTab) rec[tid] = tid == 0 ? (uint32_t)nfee : 0u;
+    if (tid < 2 * kFeeMax) {
+        const unsigned long long v = (tid >> 1) < nfee ? M.ftab[tid >> 1] : 0ull;
+        rec[kFeeTab + tid] = (uint32_t)(tid & 1 ? v >> 32 : v);
+    }
+    // pool l sits at nibble l & 7 == tid & 7 of word l >> 3: the 8 lanes of one word OR their nibbles together
+#pragma unroll
+    for (int u = 0; u < LU; ++u) {
+        unsigned code = 0;
+        for (int e = 0; e < nfee; ++e) code = M.ftab[e] == gib[u] ? (unsigned)e : code;
+        unsigned w = code << (4 * (tid & 7));
+        w |= __shfl_xor_sync(0xffffffffu, w, 1);
+        w |= __shfl_xor_sync(0xffffffffu, w, 2);
+        w |= __shfl_xor_sync(0xffffffffu, w, 4);
+        if ((tid & 7) == 0) rec[kFeeCode + ((tid + u * LT) >> 3)] = w;
     }
 }
 
@@ -203,18 +264,25 @@ k_build_tiles(const BuildArgs B) {
         }
     }
     // ---- 6. pool words and slabs, blocked order; padding pool l writes zero flows to g[l] and g[P + l], past the real ones
-    for (int l = tid; l < LP; l += LT) {
+    unsigned long long gib[LU];
+#pragma unroll
+    for (int u = 0; u < LU; ++u) {
+        const int l = tid + u * LT;
+        double gi = 1.0;
         if (l < np) {
             const uint32_t pool = B.order[p0 + l];
             B.pw[p0 + l] = (uint32_t)lidh[l][0] | (uint32_t)lidh[l][1] << 10 | (uint32_t)p1h[l] << 20;
             B.r0[p0 + l] = B.R[2 * (long long)pool]; B.r1[p0 + l] = B.R[2 * (long long)pool + 1];
-            B.gi[p0 + l] = 1.0 / B.gamma[pool];
+            gi = 1.0 / B.gamma[pool];
         } else {
             B.pw[p0 + l] = (uint32_t)l << 20;
-            B.r0[p0 + l] = 1.0; B.r1[p0 + l] = 1.0; B.gi[p0 + l] = 1.0;
+            B.r0[p0 + l] = 1.0; B.r1[p0 + l] = 1.0;
         }
+        B.gi[p0 + l] = gi;
+        gib[u] = (unsigned long long)__double_as_longlong(gi);
     }
     if (tid == 0) { B.desc[tile] = make_int4(s_ntok, nrow, 0, 0); atomicAdd(B.status + 2, nrow); }
+    if (B.fee) fee_record(B, M, tile, gib);
 }
 
 inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -238,7 +306,8 @@ int64_t cfmm_blocked_build_work_bytes(int64_t n_pools) {
 /* Build the token-blocked layout of m constant-product pools on the device.  idx [m][2] int32, reserves [m][2] f64,
  * gamma [m] f64: the reference's local_indices / reserves / fees (arbitrage.py:6-28) as contiguous device arrays.
  * `out`: a cfmm_blocked_pairs whose array members point at caller-allocated device buffers of n_tiles = ceil(m / P)
- * tiles (strides from cfmm_blocked_layout_info); r0 / r1 / gamma_inv / pw / rows / tok / desc are filled.
+ * tiles (strides from cfmm_blocked_layout_info / cfmm_blocked_fee_words); r0 / r1 / gamma_inv / pw / rows / tok / desc
+ * are filled, and the fee records if out->fee is not NULL.
  * order [m] uint32 (device, out): pool at every blocked position.  status [4] int32 (device, zeroed by this call, out):
  * [0] tiles that touch more tokens, or need more rows, than a tile may (the caller must fall back to a plain bucket for
  * such problems),
@@ -253,7 +322,6 @@ int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, co
     const long long T = (n_pools + LP - 1) / LP;
     if (out->pools_per_tile != LP || out->n_tiles != T || out->n_pools != n_pools) return CFMM_E_SIZE;
     if (!out->r0 || !out->r1 || !out->gamma_inv || !out->pw || !out->rows || !out->tok || !out->desc) return CFMM_E_NULL;
-    if (out->reserved_ptr) return CFMM_E_KIND;
     int row_cap = 32;
     cfmm_blocked_layout_info(nullptr, nullptr, nullptr, &row_cap);
     long long nb = (long long)llround(sqrt((double)n_pools / LP));
@@ -286,6 +354,7 @@ int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, co
     B.pw = const_cast<uint32_t*>(out->pw);
     B.rows = const_cast<uint32_t*>(out->rows); B.tok = const_cast<int32_t*>(out->tok);
     B.desc = reinterpret_cast<int4*>(const_cast<int32_t*>(out->desc));
+    B.fee = const_cast<uint32_t*>(out->fee);
     B.status = status;
     static bool attr = false;
     if (!attr) {

@@ -274,6 +274,41 @@ def blocked_layout_info(lib):
     return tuple(int(x.value) for x in v)      # pools_per_tile, rows_stride, tok_stride, row_cap
 
 
+def blocked_fee_words(lib) -> int:
+    """32-bit words per tile of the fee record (include/cfmm_b200.h)"""
+    return int(lib.cfmm_blocked_fee_words())
+
+
+_FEE_MAX, _FEE_TAB, _FEE_CODE = 16, 4, 36          # distinct values of a coded tile; words of the table and of the codes
+
+
+def fee_records(gamma_inv: torch.Tensor, P: int) -> torch.Tensor:
+    """Fee records (include/cfmm_b200.h) of a blocked layout from its 1/gamma slab (n_tiles * P f64, padding included):
+    per tile the header (nfee, 0, 0, 0), its distinct bit patterns in ascending order and a 4-bit index per pool into
+    them.  A tile with more than 16 distinct values gets an all-zero record: it streams its slab.
+    Returns (n_tiles, 36 + P // 8) int32."""
+    dev = gamma_inv.device
+    i64 = dict(dtype=torch.int64, device=dev)
+    bits = gamma_inv.contiguous().view(torch.int64).view(-1, P)          # positive doubles order like their bit patterns
+    T = bits.shape[0]
+    s, _ = torch.sort(bits, dim=1)
+    new = torch.ones_like(s, dtype=torch.bool)
+    new[:, 1:] = s[:, 1:] != s[:, :-1]
+    rank = torch.cumsum(new.to(torch.int64), 1) - 1                     # index of every sorted entry among the distinct
+    nfee = rank[:, -1] + 1
+    coded = (nfee <= _FEE_MAX)[:, None]
+    table = torch.zeros((T, _FEE_MAX + 1), **i64)
+    table.scatter_(1, rank.clamp(max=_FEE_MAX), s)                      # column 16 only collects tiles that are not coded
+    table = torch.where(coded, table[:, :_FEE_MAX], 0)
+    code = torch.where(coded, rank.gather(1, torch.searchsorted(s, bits)), 0)
+    words = (code.view(T, P // 8, 8) << (4 * torch.arange(8, **i64))).sum(2)
+    head = torch.zeros((T, _FEE_TAB), **i64)
+    head[:, 0] = torch.where(coded[:, 0], nfee, 0)
+    rec = torch.cat([head, table.view(torch.int32).to(torch.int64), words], 1)      # table: low word of each f64 first
+    assert rec.shape[1] == _FEE_CODE + P // 8
+    return torch.where(rec >= 2 ** 31, rec - 2 ** 32, rec).to(torch.int32).contiguous()
+
+
 def unpack_pool_words(pw: torch.Tensor, P: int):
     """Pool words of a blocked layout (``lid0 | lid1 << 10 | p1 << 20``, see csrc/cfmm_blocked.cuh) in the two-word form,
     int32 each: local ids ``lid0 | lid1 << 16`` and flow-array positions ``pos0 | pos1 << 16``, where pos0 = l (the pool's
@@ -446,7 +481,6 @@ class BlockedBucket:
         if self.m == 0:
             self.tables = None
             return
-        self.tables = t
         self.stride = t["M"]
 
         def slab(vals, fill):
@@ -456,8 +490,12 @@ class BlockedBucket:
         self.r0 = slab(R[order, 0], 1.0)
         self.r1 = slab(R[order, 1], 1.0)
         self.gamma_inv = slab(1.0 / gam[order], 1.0)
+        fee = fee_records(self.gamma_inv, P)
+        if fee.shape[1] != blocked_fee_words(lib):
+            raise _lib.CfmmError("fee record layout differs from the library's")
+        self.tables = t = BlockedTables(P, **t._t, fee=fee)
         self.c_blocked = _lib.BlockedPairs(self.m, t["n_tiles"], P, 0, self.r0.data_ptr(), self.r1.data_ptr(),
-                                           self.gamma_inv.data_ptr(), t["pw"].data_ptr(), None,
+                                           self.gamma_inv.data_ptr(), t["pw"].data_ptr(), fee.data_ptr(),
                                            t["rows"].data_ptr(), t["tok"].data_ptr(), t["desc"].data_ptr())
 
     def _build_native(self, hp, spec, device, lib, P, rows_stride, tok_stride) -> bool:
@@ -481,7 +519,11 @@ class BlockedBucket:
         slabs = torch.empty((3, M), **f64)
         pw = torch.empty(M, **i32)
         rows = torch.empty((T, rows_stride), **i32)
-        tok = torch.empty((T, tok_stride), **i32)
+        # the fee records share one allocation with the token lists: as a tensor of its own (~0.6 MB at 1M pools) they
+        # land in the caching allocator's small-block pool and shift the store's small vectors (psi, Hessian product),
+        # which made L2-hot Hessian products 23% slower on an H100
+        tok_fee = torch.empty(T * (tok_stride + blocked_fee_words(lib)), **i32)
+        tok, fee = tok_fee[:T * tok_stride].view(T, tok_stride), tok_fee[T * tok_stride:].view(T, -1)
         desc = torch.empty((T, 4), **i32)
         order = torch.empty(m, **i32)
         status = torch.empty(4, **i32)
@@ -490,7 +532,7 @@ class BlockedBucket:
             return False
         work = torch.empty(nbytes, dtype=torch.uint8, device=device)
         cb = _lib.BlockedPairs(m, T, P, 0, slabs[0].data_ptr(), slabs[1].data_ptr(), slabs[2].data_ptr(), pw.data_ptr(),
-                               None, rows.data_ptr(), tok.data_ptr(), desc.data_ptr())
+                               fee.data_ptr(), rows.data_ptr(), tok.data_ptr(), desc.data_ptr())
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         rc = lib.cfmm_blocked_build(m, hp.n_tokens, idx.data_ptr(), R.data_ptr(), gam.data_ptr(), C.byref(cb), order.data_ptr(),
                                     status.data_ptr(), work.data_ptr(), nbytes, st)
@@ -509,7 +551,7 @@ class BlockedBucket:
         self.stride = M
         self.r0, self.r1, self.gamma_inv = slabs[0], slabs[1], slabs[2]
         self._keep = (idx, R, gam, work)          # the build is asynchronous: its inputs live as long as the bucket
-        self.tables = BlockedTables(P, n_tiles=T, M=M, pw=pw, tok=tok, rows=rows, desc=desc,
+        self.tables = BlockedTables(P, n_tiles=T, M=M, pw=pw, tok=tok, rows=rows, desc=desc, fee=fee,
                                     rows_per_pool=int(st_h[2]) / m, tok_per_tile=None)
         self.c_blocked = cb
         return True
@@ -530,7 +572,7 @@ class BlockedBucket:
     def bytes_resident(self) -> int:
         if self.tables is None:
             return 0
-        ts = [self.r0, self.r1, self.gamma_inv] + [self.tables[k] for k in ("pw", "tok", "rows", "desc")]
+        ts = [self.r0, self.r1, self.gamma_inv] + [self.tables[k] for k in ("pw", "tok", "rows", "desc", "fee")]
         return sum(x.numel() * x.element_size() for x in ts)
 
     def out_struct(self, trades: bool, hess: bool):

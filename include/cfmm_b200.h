@@ -96,10 +96,21 @@ int cfmm_hess_dense(const cfmm_bucket* bucket, int32_t n_tokens, const double* h
  * Token-blocked storage for constant-product pools (the HBM-bound kind).  Built once per problem from
  * local_indices (arbitrage.py:6-12) by the layout builder (pools.py: build_blocked_pairs); pools are
  * reordered into tiles of `pools_per_tile` whose tokens fall into two narrow token blocks.  Per pool 24 B of
- * slabs + one 4 B pool word; per tile a token list, a row table and (ntok, nrow).  See csrc/cfmm_blocked.cuh.
- * Strides of the per-tile tables come from cfmm_blocked_layout_info().
+ * slabs + one 4 B pool word; per tile a token list, a row table, (ntok, nrow) and an optional fee record.  See
+ * csrc/cfmm_blocked.cuh.  Strides of the per-tile tables come from cfmm_blocked_layout_info() and
+ * cfmm_blocked_fee_words().
  * The evaluation writes the two flows of pool l of a tile to a per-tile array g[2P]: slot 0 to g[l], slot 1 to g[P + p1];
  * a row sums a contiguous run of g.
+ *
+ * Fee record of a tile (fee_words = 4 + 32 + P/8 32-bit words, a multiple of 4):
+ *   [0]        nfee: 1..16 = the tile's gamma_inv slab takes nfee distinct values ("coded" tile);
+ *              0 = more than 16 distinct values: the tile streams its gamma_inv slab and the rest of the record is zero
+ *   [1..3]     0
+ *   [4..35]    table: 16 f64, the tile's distinct gamma_inv bit patterns in ascending order (padding pools included),
+ *              zero past nfee
+ *   [36..]     codes: 4 bits per pool, pool l at bits 4 * (l & 7) of word 36 + (l >> 3)
+ * On a coded tile table[code(l)] is bit for bit the gamma_inv slab entry of pool l, and the evaluation reads it instead
+ * of the slab (7.5 B less HBM traffic per pool).  The gamma_inv slab is still required and must hold every tile's values.
  */
 typedef struct cfmm_blocked_pairs {
     int64_t n_pools;          /* real pools (<= n_tiles * pools_per_tile; the rest is padding)          */
@@ -111,13 +122,15 @@ typedef struct cfmm_blocked_pairs {
     const double* gamma_inv;  /* [n_tiles*P] 1 / fees[i]                              arbitrage.py:22-28 */
     const uint32_t* pw;       /* [n_tiles*P] pool word: tile-local token ids lid0 | lid1 << 10 | p1 << 20, each < P;
                                  p1 = rank of the slot-1 half-edge among the tile's, stably sorted by token  */
-    const void* reserved_ptr; /* must be NULL                                                             */
+    const uint32_t* fee;      /* [n_tiles][fee_words] fee records (above), or NULL: every tile streams its gamma_inv slab */
     const uint32_t* rows;     /* [n_tiles][rows_stride] start :16 | length 1..32 :6 | local token :10, longest first */
     const int32_t* tok;       /* [n_tiles][tok_stride] local token id -> global token id                 */
     const int32_t* desc;      /* [n_tiles][4] (ntok, nrow, 0, 0)                                          */
 } cfmm_blocked_pairs;
 
 int cfmm_blocked_layout_info(int32_t* pools_per_tile, int32_t* rows_stride, int32_t* tok_stride, int32_t* row_cap);
+/* 32-bit words per tile of the fee record (its stride in cfmm_blocked_pairs.fee) */
+int32_t cfmm_blocked_fee_words(void);
 /* tuning knobs for experiments: 200/201 = programmatic dependent launch off/on; 300+c = row cap c (8..32) of layouts
  * built afterwards.  (The tile size is a compile-time constant of the library, 1024 pools: the fastest of 1024 / 960 /
  * 896 for the evaluation step on an H100.) */
@@ -128,7 +141,8 @@ int cfmm_set_blocked_config(int32_t cfg);
  * [m][2] f64, fees as gamma [m] f64 (arbitrage.py:6-28), contiguous on the device -- become the blocked layout in three
  * launches (pool keys + validation, radix sort, one CTA per tile).  `out`: a cfmm_blocked_pairs with n_pools = m,
  * n_tiles = ceil(m / P), pools_per_tile = P whose array members point at caller-allocated device buffers (strides from
- * cfmm_blocked_layout_info; slabs / pw of n_tiles * P entries); all of them are filled.  order [m] uint32 (out):
+ * cfmm_blocked_layout_info; slabs / pw of n_tiles * P entries); all of them are filled, and so are the fee records if
+ * `fee` is not NULL.  order [m] uint32 (out):
  * the pool at every blocked position.  status [4] int32 (device, out): [0] tiles that touch more tokens, or need more
  * rows, than a tile may (then the layout is unusable: use a plain bucket), [1] != 0: invalid pools (reserves <= 0 or not finite, fees outside
  * (0, 1], token ids out of range or equal), [2] rows in total.  CFMM_E_SIZE if the sort keys would not fit 32 bits
