@@ -118,6 +118,10 @@ def load(build_if_missing: bool = True):
     lib.cfmm_blocked_build_work_bytes.restype = i64
     lib.cfmm_blocked_build.argtypes = [i64, i32, vp, vp, vp, C.POINTER(BlockedPairs), vp, vp, vp, i64, vp]
     lib.cfmm_blocked_build.restype = C.c_int
+    lib.cfmm_blocked_update_work_bytes.argtypes = [C.POINTER(BlockedPairs)]
+    lib.cfmm_blocked_update_work_bytes.restype = i64
+    lib.cfmm_blocked_update.argtypes = [C.POINTER(BlockedPairs), i64, vp, vp, vp, C.POINTER(i32), vp, i64, vp]
+    lib.cfmm_blocked_update.restype = C.c_int
     lib.cfmm_blocked_eval.argtypes = [C.POINTER(BlockedPairs), i32, vp, vp, vp, C.POINTER(EvalOut), vp, i64, vp]
     lib.cfmm_blocked_eval.restype = C.c_int
     lib.cfmm_blocked_hvp.argtypes = [C.POINTER(BlockedPairs), i32, vp, vp, vp, vp, vp]

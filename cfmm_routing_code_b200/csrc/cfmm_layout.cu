@@ -70,6 +70,11 @@ k_pool_keys(long long m, int n_tokens, int nb, const int32_t* __restrict__ idx, 
 using Sort = cub::BlockRadixSort<uint32_t, LT, LI, uint32_t>;
 using Scan = cub::BlockScan<int, LT>;
 
+struct FeeSmem {                           // shared memory of fee_record (a tile CTA of the builder or of the refresh)
+    unsigned long long wmin[LT / 32];      // per-warp minima of a block min
+    unsigned long long ftab[kFeeMax];      // the tile's distinct 1/gamma bit patterns, ascending
+};
+
 struct TileSmem {                          // dynamic shared memory of one tile CTA (> 48 KB with the cub scratch)
     union { typename Sort::TempStorage sort; typename Scan::TempStorage scan; } tmp;
     uint32_t sk[LH];                       // half-edges sorted by token: token id
@@ -79,8 +84,7 @@ struct TileSmem {                          // dynamic shared memory of one tile 
     uint16_t rlen[LH];                     // length of the run of equal tokens that starts at a position of the flow array
     uint16_t lidh[LP][2], p1h[LP];         // local ids and slot-1 position of every pool
     int ntok;
-    unsigned long long wmin[LT / 32];      // per-warp minima of a block min
-    unsigned long long ftab[kFeeMax];      // the tile's distinct 1/gamma bit patterns, ascending
+    FeeSmem fs;
 };
 
 // a tile the layout cannot hold: counted in status[0], its slabs and tables kept inert (never launched: the host falls back)
@@ -95,7 +99,7 @@ __device__ void inert_tile(const BuildArgs& B, long long tile) {
 }
 
 // minimum over the tile CTA (every thread gets it)
-__device__ unsigned long long block_min(unsigned long long x, TileSmem& M) {
+__device__ unsigned long long block_min(unsigned long long x, FeeSmem& M) {
     for (int o = 16; o > 0; o >>= 1) {
         const unsigned long long y = __shfl_xor_sync(0xffffffffu, x, o);
         x = y < x ? y : x;
@@ -108,12 +112,12 @@ __device__ unsigned long long block_min(unsigned long long x, TileSmem& M) {
     return x;
 }
 
-// ---- 7. fee record (include/cfmm_b200.h) of a tile whose pool l = tid + u * LT has 1/gamma bit pattern gib[u], padding
-// included: the distinct patterns in ascending order, one block min over the patterns above the last one per value
-// (positive doubles order like their bit patterns), then a 4-bit index per pool.  More than kFeeMax values: all zero.
-__device__ void fee_record(const BuildArgs& B, TileSmem& M, long long tile, const unsigned long long (&gib)[LU]) {
+// ---- 7. fee record `rec` (include/cfmm_b200.h) of a tile whose pool l = tid + u * LT has 1/gamma bit pattern gib[u],
+// padding included: the distinct patterns in ascending order, one block min over the patterns above the last one per
+// value (positive doubles order like their bit patterns), then a 4-bit index per pool.  More than kFeeMax values: all
+// zero.  Shared by the builder (k_build_tiles) and the in-place update (k_refresh_fees).
+__device__ void fee_record(uint32_t* rec, FeeSmem& M, const unsigned long long (&gib)[LU]) {
     const int tid = threadIdx.x;
-    uint32_t* rec = B.fee + tile * LF;
     unsigned long long last = 0;
     int nfee = 0;
     bool over = false;
@@ -282,7 +286,56 @@ k_build_tiles(const BuildArgs B) {
         gib[u] = (unsigned long long)__double_as_longlong(gi);
     }
     if (tid == 0) { B.desc[tile] = make_int4(s_ntok, nrow, 0, 0); atomicAdd(B.status + 2, nrow); }
-    if (B.fee) fee_record(B, M, tile, gib);
+    if (B.fee) fee_record(B.fee + tile * LF, M.fs, gib);
+}
+
+// ---- in-place update of a built layout (cfmm_blocked_update).  The layout depends on the token ids only; reserves and
+// fees are payload: new values go to their blocked positions, and the fee record of every tile whose 1/gamma slab
+// changed is rebuilt from the slab by fee_record, so the result is bit for bit what the builder makes of the new data.
+// status[0]: invalid entries (the rules of k_pool_keys), status[1]: fee records rebuilt.
+__global__ void __launch_bounds__(256)
+k_update_check(long long n, long long n_pools, const uint32_t* __restrict__ at, const double* __restrict__ R,
+               const double* __restrict__ gamma, int32_t* status) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        bool ok = at[i] < n_pools;
+        if (R) {
+            const double R0 = R[2 * i], R1 = R[2 * i + 1];
+            ok = ok && R0 > 0.0 && R1 > 0.0 && isfinite(R0) && isfinite(R1);
+        }
+        if (gamma) {
+            const double g = gamma[i];
+            ok = ok && g > 0.0 && g <= 1.0;
+        }
+        if (!ok) atomicAdd(status, 1);
+    }
+}
+
+// applies the update only if k_update_check found nothing wrong; flags the tile of every pool whose 1/gamma changed
+__global__ void __launch_bounds__(256)
+k_update_apply(long long n, const uint32_t* __restrict__ at, const double* __restrict__ R, const double* __restrict__ gamma,
+               double* r0, double* r1, double* gi, uint32_t* flag, const int32_t* status) {
+    if (*status != 0) return;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long p = at[i];
+        if (R) { r0[p] = R[2 * i]; r1[p] = R[2 * i + 1]; }
+        if (gamma) {
+            const double g = 1.0 / gamma[i];                            // the builder's division
+            if (__double_as_longlong(g) != __double_as_longlong(gi[p])) { gi[p] = g; flag[p / LP] = 1u; }
+        }
+    }
+}
+
+// one CTA per tile: a flagged tile rebuilds its fee record from its 1/gamma slab
+__global__ void __launch_bounds__(LT)
+k_refresh_fees(const double* __restrict__ gi, uint32_t* fee, const uint32_t* __restrict__ flag, int32_t* status) {
+    __shared__ FeeSmem M;
+    const long long tile = blockIdx.x;
+    if (flag[tile] == 0u) return;
+    unsigned long long gib[LU];
+#pragma unroll
+    for (int u = 0; u < LU; ++u) gib[u] = (unsigned long long)__double_as_longlong(gi[tile * LP + threadIdx.x + u * LT]);
+    fee_record(fee + tile * LF, M, gib);
+    if (threadIdx.x == 0) atomicAdd(status + 1, 1);
 }
 
 inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -363,6 +416,53 @@ int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, co
     }
     k_build_tiles<<<(int)T, LT, sizeof(TileSmem), st>>>(B);
     return check_launch();
+}
+
+/* work of cfmm_blocked_update: the two status words, then one flag per tile */
+int64_t cfmm_blocked_update_work_bytes(const cfmm_blocked_pairs* b) {
+    if (!b) return CFMM_E_NULL;
+    if (b->n_tiles < 0) return CFMM_E_SIZE;
+    return (int64_t)(align_up(8) + align_up(4 * (size_t)b->n_tiles));
+}
+
+/* In-place update of the reserves and fees of n_upd pools of a built layout (include/cfmm_b200.h).  Check, apply (only
+ * if the check found nothing), refresh the fee records of the tiles whose 1/gamma changed; then wait for the stream. */
+int cfmm_blocked_update(const cfmm_blocked_pairs* b, int64_t n_upd, const uint32_t* at, const double* reserves,
+                        const double* gamma, int32_t* status_host, void* work, int64_t work_bytes, void* stream) {
+    if (!b || !status_host) return CFMM_E_NULL;
+    if (n_upd < 0 || b->n_tiles < 0 || b->n_pools < 0 || b->n_pools > b->n_tiles * (int64_t)LP) return CFMM_E_SIZE;
+    if (b->pools_per_tile != LP) return CFMM_E_KIND;
+    status_host[0] = status_host[1] = 0;
+    if (n_upd == 0) return CFMM_OK;
+    if (!at || !work || !b->r0 || !b->r1 || !b->gamma_inv) return CFMM_E_NULL;
+    if (work_bytes < cfmm_blocked_update_work_bytes(b)) return CFMM_E_SIZE;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int32_t* status = static_cast<int32_t*>(work);
+    uint32_t* flag = reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(work) + align_up(8));
+    // the whole work buffer is cleared here, so it needs no initialisation and may be shared between layouts
+    if (cudaMemsetAsync(work, 0, (size_t)cfmm_blocked_update_work_bytes(b), st) != cudaSuccess) {
+        g_last_err = cudaGetLastError();
+        return CFMM_E_CUDA;
+    }
+    const int grid = (int)((n_upd + 255) / 256 < 4LL * num_sms() ? (n_upd + 255) / 256 : 4LL * num_sms());
+    k_update_check<<<grid, 256, 0, st>>>(n_upd, b->n_pools, at, reserves, gamma, status);
+    int rc = check_launch();
+    if (rc) return rc;
+    k_update_apply<<<grid, 256, 0, st>>>(n_upd, at, reserves, gamma, const_cast<double*>(b->r0), const_cast<double*>(b->r1),
+                                         const_cast<double*>(b->gamma_inv), flag, status);
+    rc = check_launch();
+    if (rc) return rc;
+    if (gamma && b->fee && b->n_tiles > 0) {
+        k_refresh_fees<<<(int)b->n_tiles, LT, 0, st>>>(b->gamma_inv, const_cast<uint32_t*>(b->fee), flag, status);
+        rc = check_launch();
+        if (rc) return rc;
+    }
+    if (cudaMemcpyAsync(status_host, status, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) {
+        g_last_err = cudaGetLastError();
+        return CFMM_E_CUDA;
+    }
+    return CFMM_OK;
 }
 
 }  // extern "C"

@@ -108,6 +108,75 @@ class HostPools:
             raise ValueError("token index out of range")
 
 
+@dataclasses.dataclass
+class PoolUpdate:
+    """A checked update of some pools' reserves and fees (check_pool_update)."""
+    ids: np.ndarray                  # int64 [n] global pool indices
+    ptr: np.ndarray                  # int64 [n+1] pool k's slots are slots[ptr[k]:ptr[k+1]]
+    slots: np.ndarray                # int64 [nnz] CSR offsets of the updated pools' slots, pool by pool, in slot order
+    reserves: Optional[np.ndarray]   # f64 [nnz] new reserves at `slots`, or None
+    gamma: Optional[np.ndarray]      # f64 [n] new fees, or None
+
+
+def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarray, pool_ids, reserves=None,
+                      fees=None) -> PoolUpdate:
+    """Host checks of PoolStore.update_pools, on the problem's CSR arrays (pool_ptr, kind, weights as in HostPools).
+    pool_ids: global pool indices, distinct and in range; reserves[k]: the new reserve vector of pool pool_ids[k] with the
+    pool's arity (a row of the reference's `reserves` literal; an (n, k) array when all pools have arity k); fees[k]: its
+    new gamma.  The values must pass the rules of HostPools.validate (bounded_product pools with their own offsets).
+    Raises ValueError; returns the update with the reserves flattened into the pools' CSR slot order."""
+    m = len(pool_ptr) - 1
+    ids = np.asarray(pool_ids)
+    if ids.ndim != 1 or (ids.size and not np.issubdtype(ids.dtype, np.integer)):
+        raise ValueError("pool_ids must be a 1-d sequence of integer pool indices")
+    ids = ids.astype(np.int64)
+    n = len(ids)
+    if reserves is None and fees is None:
+        raise ValueError("nothing to update: give reserves, fees or both")
+    if n and (ids.min() < 0 or ids.max() >= m):
+        raise ValueError(f"pool id out of range [0, {m})")
+    srt = np.sort(ids)                                   # (np.unique hashes: 20x slower at 100k ids)
+    if bool(np.any(srt[1:] == srt[:-1])):
+        raise ValueError("repeated pool id")
+    if int(pool_ptr[-1]) == 2 * m:       # every pool of a store has >= 2 tokens, so these are all pairs: no gathers
+        ar = np.full(n, 2, np.int64)
+        first = 2 * np.arange(n + 1, dtype=np.int64)
+        slots = (2 * ids[:, None] + np.arange(2)).reshape(-1)
+    else:
+        ar = (pool_ptr[ids + 1] - pool_ptr[ids]).astype(np.int64)
+        first = np.concatenate([[0], np.cumsum(ar)])
+        slots = np.repeat(pool_ptr[ids] - first[:-1], ar) + np.arange(first[-1], dtype=np.int64)
+    R = None
+    if reserves is not None:
+        if isinstance(reserves, np.ndarray) and reserves.ndim == 2:
+            if len(reserves) != n or (n and bool(np.any(ar != reserves.shape[1]))):
+                raise ValueError("reserves: one row per pool, of the pool's arity")
+            R = np.ascontiguousarray(reserves, np.float64).reshape(-1)
+        else:
+            if len(reserves) != n:
+                raise ValueError("reserves: one vector per pool")
+            rows = [np.asarray(r, np.float64).reshape(-1) for r in reserves]
+            if any(len(r) != a for r, a in zip(rows, ar.tolist())):
+                raise ValueError("reserves: a vector's length differs from its pool's arity")
+            R = np.concatenate(rows) if rows else np.zeros(0)
+        bounded = np.repeat(np.asarray(kind)[ids] == KIND_BOUNDED_HOST, ar)
+        if bounded.any():
+            virt = R + np.where(bounded, weights[slots], 0.0)
+            ok = np.where(bounded, R >= 0, True) & (virt > 0)
+        else:
+            ok = R > 0
+        if not (bool(np.all(ok)) and bool(np.all(np.isfinite(R)))):
+            raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves)")
+    g = None
+    if fees is not None:
+        g = np.ascontiguousarray(fees, np.float64).reshape(-1)
+        if len(g) != n:
+            raise ValueError("fees: one per pool")
+        if not bool(np.all((g > 0) & (g <= 1))):
+            raise ValueError("fees (gamma) must lie in (0, 1]")
+    return PoolUpdate(ids, first, slots, R, g)
+
+
 class BucketSpec:
     """Which pools of a HostPools form one bucket.  `sel` = global pool indices (None = all pools, in order,
     the fast path for constant-product-only problems: no host-side gathers at all)."""
@@ -248,6 +317,19 @@ class DeviceBucket:
     @property
     def off(self) -> np.ndarray:
         return self.spec.off
+
+    def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
+                     W: Optional[np.ndarray] = None):
+        """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
+        Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__."""
+        f64 = dict(dtype=torch.float64, device=self._device)
+        li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
+        if R is not None:
+            self.reserves[:, li] = torch.as_tensor(R, **f64)
+            if self.logrw is not None:
+                self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
+        if gamma is not None:
+            self.gamma[li] = torch.as_tensor(gamma, **f64)
 
     def bytes_resident(self) -> int:
         n = 0
@@ -569,6 +651,30 @@ class BlockedBucket:
             self._off = self.spec.hp.pool_ptr[self.sel][None, :] + np.arange(2)[:, None]
         return self._off
 
+    def write_update(self, lib, pos: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray], stream) -> int:
+        """cfmm_blocked_update: new reserves R (2, n) and / or fees (n,) of the pools at blocked positions `pos`.  Checks
+        every entry on the device and writes nothing if one is invalid (ValueError).  Synchronous.  Returns the number
+        of fee records rebuilt."""
+        dev = self._device
+        at = torch.as_tensor(np.asarray(pos, np.uint32).view(np.int32), device=dev)
+        Rd = None if R is None else torch.as_tensor(np.ascontiguousarray(R.T), dtype=torch.float64, device=dev)
+        gd = None if gamma is None else torch.as_tensor(gamma, dtype=torch.float64, device=dev)
+        if getattr(self, "_upd_work", None) is None:
+            nbytes = int(lib.cfmm_blocked_update_work_bytes(C.byref(self.c_blocked)))
+            if nbytes < 0:
+                _lib.check(nbytes, "cfmm_blocked_update_work_bytes")
+            self._upd_work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        status = (C.c_int32 * 2)()
+        _lib.check(lib.cfmm_blocked_update(C.byref(self.c_blocked), len(pos), at.data_ptr(),
+                                           Rd.data_ptr() if Rd is not None else None,
+                                           gd.data_ptr() if gd is not None else None, status,
+                                           self._upd_work.data_ptr(), self._upd_work.numel(), stream),
+                   "cfmm_blocked_update")
+        if status[0] != 0:
+            raise ValueError(f"{status[0]} invalid pool update(s) (reserves > 0 and finite, fees in (0, 1]); "
+                             "nothing was written")
+        return int(status[1])
+
     def bytes_resident(self) -> int:
         if self.tables is None:
             return 0
@@ -662,6 +768,8 @@ class PoolStore:
         self.m_total = hp.m
         self.pool_ptr = hp.pool_ptr
         self._tok_idx_host = hp.tok_idx
+        self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets
+        self._where = None                                               # pool -> (bucket, position): update_pools
         self.rank, self.world = rank, world
         self.buckets = []
         for s in split_buckets(hp, rank, world):
@@ -816,6 +924,59 @@ class PoolStore:
         for b in self.buckets:
             if b.theta_bar is not None:
                 b.theta_bar.zero_()
+
+    # -- a changed market: new reserves / fees in place ------------------------------------------------
+    def _pool_map(self):
+        """(bucket index or -1, position in that bucket) of every global pool id, built once per store"""
+        if self._where is None:
+            bi = np.full(self.m_total, -1, np.int32)
+            loc = np.zeros(self.m_total, np.int64)
+            for k, b in enumerate(self.buckets):
+                s = b.sel                # blocked bucket: the pool at every blocked position (the inverse of its order)
+                bi[s] = k
+                loc[s] = np.arange(len(s))
+            self._where = (bi, loc)
+        return self._where
+
+    def update_pools(self, pool_ids, reserves=None, fees=None):
+        """Set new reserves and / or fees of some pools in place: the store then equals, bit for bit, a PoolStore built
+        from the updated host data, without re-uploading the pools or rebuilding the blocked layout (which depends on the
+        token ids only).  pool_ids: global pool indices (the order of the problem's local_indices); reserves[k]: the new
+        reserve vector of pool pool_ids[k], with the pool's arity (an (n, 2) array for pairs); fees[k]: its new gamma in
+        (0, 1].  At least one of reserves / fees.  Kinds, tokens, weights and bounded_product offsets cannot change.
+
+        All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.validate) raise
+        ValueError before anything is written, and so does an entry the device check of the blocked bucket rejects.
+        Pools held by other ranks of a sharded store are skipped: give every rank the same full update.  The caller's
+        HostPools is not modified (the store reads no host reserve or fee after construction).  Synchronous.  Returns
+        the number of blocked tiles whose fee record was rebuilt.
+
+        A new block of the same market is then re-solved warm from the previous prices:
+            store.update_pools(ids, reserves=new_R, fees=new_gamma)
+            res = solve_pools(hp, utility, store=store, nu0=res.nu)"""
+        u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees)
+        bi, loc = self._pool_map()
+        owner = bi[u.ids]
+        plan = []
+        for k, b in enumerate(self.buckets):
+            e = np.nonzero(owner == k)[0]
+            if len(e) == 0:
+                continue
+            rs = u.ptr[e][None, :] + np.arange(b.arity)[:, None]          # (arity, n) indices into the update's slots
+            R = None if u.reserves is None else u.reserves[rs]
+            g = None if u.gamma is None else u.gamma[e]
+            plan.append((b, loc[u.ids[e]], R, g, rs))
+        # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
+        rebuilt = 0
+        for b, l, R, g, _ in plan:
+            if getattr(b, "blocked", False):
+                rebuilt += b.write_update(self.lib, l, R, g, self._stream())
+        for b, l, R, g, rs in plan:
+            if not getattr(b, "blocked", False):
+                W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None) else None
+                b.write_update(l, R, g, W)
+        torch.cuda.synchronize(self.device)
+        return rebuilt
 
     def gather_trades(self):
         """Delta, Lambda of the last trades=True evaluation, CSR order of the ORIGINAL pools (host).

@@ -153,6 +153,29 @@ int cfmm_blocked_build(int64_t n_pools, int32_t n_tokens, const int32_t* idx, co
                        const cfmm_blocked_pairs* out, uint32_t* order, int32_t* status, void* work, int64_t work_bytes,
                        void* stream);
 
+/*
+ * In-place update of the reserves and fees of n_upd pools of a built blocked layout (a new block of the same market: the
+ * layout depends on the token ids only, reserves and fees are payload).  at [n_upd] uint32: BLOCKED positions
+ * (< b->n_pools; the builder's `order` maps position -> pool, the caller inverts it once).  reserves [n_upd][2] f64: new
+ * R0, R1 in the pool's own slot order, or NULL; gamma [n_upd] f64: new fees, or NULL.  Positions must be distinct
+ * (with repeats one of the values wins; the fee records stay consistent with the slab).
+ * All or nothing: one launch checks every entry (position in range, reserves > 0 and finite, fee in (0, 1], the rules
+ * of cfmm_blocked_build); only if none is invalid does a second launch write r0 / r1 and gamma_inv = 1.0 / gamma (the
+ * builder's IEEE division), and a third rebuild the fee record of every tile whose gamma_inv slab changed (if b->fee is
+ * not NULL).  The layout then equals, bit for bit, what cfmm_blocked_build makes of the updated data.
+ * status_host [2] int32 (host, out): [0] invalid entries (nothing was written if > 0), [1] fee records rebuilt.
+ * work: cfmm_blocked_update_work_bytes(b) bytes of device memory, cleared by every call (no initialisation needed).
+ * SYNCHRONOUS on `stream`: the call returns after the stream has drained.  This is deliberate: the standalone blocked
+ * kernels issue the bulk copies of their first tiles before they wait for the previous grid (programmatic dependent
+ * launch), so an evaluation queued right behind the update kernels could stream the old r0 / r1 / fee record of its
+ * first tiles.  Not capturable in a CUDA graph.
+ * Plain buckets (cfmm_bucket) need no entry point: their slot-major arrays belong to the caller, who writes them
+ * directly (for GEOMEAN pools keep logrw = log(reserves / weights) in step).
+ */
+int64_t cfmm_blocked_update_work_bytes(const cfmm_blocked_pairs* b);
+int cfmm_blocked_update(const cfmm_blocked_pairs* b, int64_t n_upd, const uint32_t* at, const double* reserves,
+                        const double* gamma, int32_t* status_host, void* work, int64_t work_bytes, void* stream);
+
 /* Same contract as cfmm_arb_eval for a blocked constant-product bucket: psi/arb ACCUMULATE (one red.add per row
  * of <= 32 entries, ~0.35 per pool, instead of 2 per pool).  Per-pool outputs (delta/lambda [2][n_tiles*P], hcoef
  * [n_tiles*P]) are in BLOCKED order.  If zero_next != NULL the launch also clears zero_next[0..n_zero): callers that
