@@ -14,6 +14,8 @@ extern thread_local cudaError_t g_last_err;
 
 int num_sms();
 
+constexpr double kDtMax = 3.0;      // largest log-price change of one Newton step (solver.py DT_MAX, cfmm_small.cuh DT_MAX)
+
 inline int check_launch() {
     g_launches.fetch_add(1, std::memory_order_relaxed);
     cudaError_t e = cudaGetLastError();

@@ -119,7 +119,7 @@ struct DistArgs {
 
 struct DState {                                  // replicated in every CTA's shared memory; thread 0 updates it
     int phase, set, cur, iters, evals, hvps, status, cg_k, ls, yb, first_step, dir_ok, aborted, parity;
-    double err, g0, rz, r0n, eta, alpha, lin1, beta, al, imx, thr;
+    double err, g0, rz, r0n, eta, alpha, lin1, beta, al, imx, thr, dsc;
     int flat;
     Kkt kc;
     unsigned long long seq_acc, seq_vec;
@@ -203,7 +203,7 @@ k_solve_dist(const __grid_constant__ DistArgs D) {
         ds.phase = PH_KKT; ds.set = 0; ds.cur = 0; ds.iters = 0; ds.evals = 0; ds.hvps = 0; ds.status = 1; ds.cg_k = 0; ds.ls = 0;
         ds.yb = 0; ds.first_step = 1; ds.dir_ok = 0; ds.aborted = 0; ds.parity = 0; ds.flat = 0;
         ds.err = INFINITY; ds.g0 = 0.0; ds.rz = 0.0; ds.r0n = 0.0; ds.eta = 0.1; ds.alpha = 1.0; ds.lin1 = 0.0; ds.beta = 0.0;
-        ds.al = 0.0; ds.imx = 0.0; ds.thr = 1e-5;
+        ds.al = 0.0; ds.imx = 0.0; ds.thr = 1e-5; ds.dsc = 1.0;
         ds.kc.err = INFINITY; ds.kc.g = 0.0; ds.kc.primal = 0.0; ds.kc.infeas = 0.0; ds.kc.lin = 0.0;
         ds.seq_acc = S.seq_acc; ds.seq_vec = S.seq_vec; ds.bar = 0;
         for (int k = 0; k < 16; ++k) ds.prof[k] = 0;
@@ -322,11 +322,12 @@ k_solve_dist(const __grid_constant__ DistArgs D) {
                         q[0] += r * z;
                     }
                     q[1] += g * xn;                  // pg . x: is x a descent direction (needed when PCG stops here)
+                    q[6] = fmax(q[6], fabs(xn));     // max |x|: the step is bounded to kDtMax when PCG stops here
                     D.y2[ds.yb ^ 1][j] = 0.0;
                 } else {                             // PH_STEP: direction (first step of a search) + trial point
                     const double g = ldw(S.pg[cur] + j), xx = ldw(S.x + j), v = ldw(S.nu[cur] + j), l = ldw(S.lb + j);
                     double d;
-                    if (ds.first_step) { d = ds.dir_ok ? xx : -g * ds.imx; S.dt[j] = d; }
+                    if (ds.first_step) { d = ds.dir_ok ? xx * ds.dsc : -g * ds.imx; S.dt[j] = d; }
                     else d = ldw(S.dt + j);
                     const double e = fmin(fmax(ds.alpha * d, -20.0), 20.0);
                     S.nu[cur ^ 1][j] = S.fixed[j] ? S.c[j] : fmax(v * exp(e), l);
@@ -422,6 +423,9 @@ k_solve_dist(const __grid_constant__ DistArgs D) {
                 else {
                     const double sdir = tot[1];
                     ds.dir_ok = (isfinite(sdir) && sdir < 0.0) ? 1 : 0;
+                    // at most kDtMax per coordinate, as solver.py bounds it: a truncated-CG step can be ~1e14 long, and
+                    // every trial of the search would then sit on the +-20 clamp of PH_STEP
+                    ds.dsc = tot[6] > kDtMax ? kDtMax / tot[6] : 1.0;
                     ds.first_step = 1; ds.alpha = 1.0; ds.ls = 0; ds.lin1 = 0.0;
                     next = PH_STEP;
                 }

@@ -153,14 +153,19 @@ __global__ void __launch_bounds__(kVT) k_cg_step(Vecs V, const double* y, double
     if (threadIdx.x == 0) { V.sc[S_RZ] = rzn; V.sc[S_STOP] = done ? 1.0 : 0.0; }
 }
 
-// dt <- x if it is a descent direction in value units (pg . dt < 0), else scaled steepest descent
+// dt <- x if it is a descent direction in value units (pg . dt < 0), else scaled steepest descent; then at most kDtMax
+// in every coordinate (solver.py DT_MAX: a truncated-CG step can be ~1e14 long, and every trial of the search would sit
+// on k_step's +-20 clamp)
 __global__ void __launch_bounds__(kVT) k_direction(Vecs V) {
     __shared__ double sh[33];
-    double s = 0, mx = 0;
-    for (int j = threadIdx.x; j < V.n; j += kVT) { s += V.pg[j] * V.x[j]; mx = fmax(mx, fabs(V.pg[j])); }
-    s = block_sum(s, sh); mx = block_max(mx, sh);
+    double s = 0, mx = 0, xm = 0;
+    for (int j = threadIdx.x; j < V.n; j += kVT) {
+        s += V.pg[j] * V.x[j]; mx = fmax(mx, fabs(V.pg[j])); xm = fmax(xm, fabs(V.x[j]));
+    }
+    s = block_sum(s, sh); mx = block_max(mx, sh); xm = block_max(xm, sh);
     const bool ok = isfinite(s) && s < 0.0;
-    for (int j = threadIdx.x; j < V.n; j += kVT) V.dt[j] = ok ? V.x[j] : -V.pg[j] / fmax(mx, 1e-300);
+    const double sc = ok && xm > kDtMax ? kDtMax / xm : 1.0;       // steepest descent is at most 1 long already
+    for (int j = threadIdx.x; j < V.n; j += kVT) V.dt[j] = ok ? V.x[j] * sc : -V.pg[j] / fmax(mx, 1e-300);
     if (threadIdx.x == 0) V.sc[S_SLOPE] = s;
 }
 

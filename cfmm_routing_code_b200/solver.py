@@ -28,7 +28,7 @@ import numpy as np
 import torch
 
 
-DT_MAX = 3.0      # largest log-price change of one dense Newton step
+DT_MAX = 3.0      # largest log-price change of one Newton step (dense or CG)
 LM_SHIFTS = (1e-14, 1e-8, 1e-6, 1e-4, 1e-2, 1.0)     # damping ladder of the dense Newton system, times the mean diagonal
 
 
@@ -228,12 +228,13 @@ def solve_dual(ev, spec: DualSpec, nu0=None, tol: float = 1e-8, eps: float = 0.1
                 slope = torch.dot(pg, dt)     # = grad . (nu*dt)
                 if not bool(torch.isfinite(slope)) or float(slope) >= 0.0:
                     dt = -pg / pg.abs().max().clamp(min=1e-300)
-                if linear_solver == "dense":
-                    # (near-)singular system, e.g. every pool tying the free prices to a bound is saturated: keep the
-                    # direction, bound the step to a price factor of e^3 and let the line search find the kink
-                    big = float(dt.abs().max())
-                    if big > DT_MAX:
-                        dt = dt * (DT_MAX / big)
+                # (near-)singular system, e.g. every pool tying the free prices to a bound is saturated: keep the
+                # direction, bound the step to a price factor of e^3 and let the line search find the kink.  A truncated-CG
+                # step can be as long (a swap over 65 536 tokens gave one of ~1e14): unbounded, every trial of the search
+                # sits on the +-20 clamp below -- the same point -- until the 50 halvings run out
+                big = float(dt.abs().max())
+                if big > DT_MAX:
+                    dt = dt * (DT_MAX / big)
                 # ---- projected Armijo backtracking along nu * exp(alpha dt)
                 alpha = 1.0
                 g0 = float(g)
