@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .pools import HostPools, KIND_GEOMEAN_HOST
+from .pools import HostPools, KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
 from .solver import default_nu0
 
 NTOK_MAX = 64      # cfmm_small::NTOK_MAX
@@ -48,6 +48,12 @@ class CsrStore:
         self.R = torch.as_tensor(np.ascontiguousarray(hp.reserves, np.float64), device=dev)
         self.w = torch.as_tensor(np.ascontiguousarray(hp.weights, np.float64), device=dev)
         self.logrw = torch.log(torch.clamp(self.R, min=1e-300) / torch.as_tensor(w, device=dev))
+        ss = np.nonzero(np.asarray(hp.kind) == KIND_STABLESWAP_HOST)[0]
+        self.has_stableswap = bool(len(ss))         # -> cfmm_batch_solve_stableswap (its own kernel instance)
+        if len(ss):                                  # StableSwap pools: A at the first slot, the invariant D at the second
+            first = torch.as_tensor(np.asarray(hp.pool_ptr)[ss], device=dev)
+            self.logrw[first] = torch.as_tensor(np.asarray(hp.amp, np.float64)[ss], device=dev)
+            self.logrw[first + 1] = torch.as_tensor(np.asarray(hp.inv, np.float64)[ss], device=dev)
         self.gamma = torch.as_tensor(np.ascontiguousarray(hp.gamma, np.float64), device=dev)
         self.kind = torch.as_tensor(np.ascontiguousarray(hp.kind, np.uint8), device=dev)
         self.c_pools = _lib.CsrPools(self.n_tokens, self.m, self.nnz, self.pool_ptr.data_ptr(), self.tok.data_ptr(),
@@ -100,8 +106,8 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(store.lib.cfmm_batch_solve(C.byref(store.c_pools), C.byref(batch), C.byref(prm), work.data_ptr(), st),
-               "cfmm_batch_solve")
+    entry = store.lib.cfmm_batch_solve_stableswap if store.has_stableswap else store.lib.cfmm_batch_solve
+    _lib.check(entry(C.byref(store.c_pools), C.byref(batch), C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve")
     return psi, stats, delta, lam
 
 
@@ -178,7 +184,8 @@ def pack_problems(problems: Sequence):
         c[p, k:] = 1.0
     cat = lambda name, dt: np.concatenate([np.asarray(getattr(hp, name), dt) for hp, _ in problems])
     merged = HostPools(n, np.concatenate(ptr), cat("tok_idx", np.int32), cat("reserves", np.float64),
-                       cat("weights", np.float64), cat("gamma", np.float64), cat("kind", np.uint8))
+                       cat("weights", np.float64), cat("gamma", np.float64), cat("kind", np.uint8),
+                       cat("amp", np.float64), cat("inv", np.float64))
     return merged, ranges, c, a, fl, nu, nnz_max
 
 

@@ -175,6 +175,37 @@ k_eval_pair(long long m, long long ld, int n_tokens, const double* __restrict__ 
     block_accumulate(acc, arb);
 }
 
+// two-coin StableSwap: cfmm_small::stableswap_pair (a safeguarded Newton solve per trading pool, compute-bound rather
+// than HBM-bound), one thread per pool.  rates [2][ld] (the bucket's weights), AD [2][ld] = (A, D) (the bucket's logrw).
+template <typename Scatter, bool TRADES, bool HESS>
+__global__ void __launch_bounds__(kThreads)
+k_eval_stable(long long m, long long ld, int n_tokens, const double* __restrict__ R, const int* __restrict__ idx,
+              const double* __restrict__ gamma, const double* __restrict__ rates, const double* __restrict__ AD,
+              const double* __restrict__ nu, double* psi, double* arb, double* delta, double* lambda, double* hcoef) {
+    extern __shared__ double smem[];
+    Scatter sc{psi};
+    sc.init(smem, n_tokens);
+    double acc = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        const int i0 = idx[i], i1 = idx[ld + i];
+        const double n0 = __ldg(nu + i0), n1 = __ldg(nu + i1);
+        double D[2], L[2], h;
+        cfmm_small::stableswap_pair(R[i], R[ld + i], rates[i], rates[ld + i], AD[i], AD[ld + i], gamma[i], n0, n1, D, L, h);
+        const double y0 = L[0] - D[0], y1 = L[1] - D[1];
+        if (TRADES) {
+            delta[i] = D[0]; delta[ld + i] = D[1];
+            lambda[i] = L[0]; lambda[ld + i] = L[1];
+        }
+        if (HESS) hcoef[i] = h;
+        if (y0 != 0.0) sc.add(i0, y0);
+        if (y1 != 0.0) sc.add(i1, y1);
+        acc += n0 * y0 + n1 * y1;
+    }
+    sc.flush(smem, n_tokens);
+    block_accumulate(acc, arb);
+}
+
 // ---------------------------------------------------------------------------------------------
 // TMA-staged variant of the 2-token kernel: persistent CTAs, each walking tiles of kTile pools.
 // One elected thread issues five 1-D bulk copies per tile (cp.async.bulk -> UBLKCP: R0, R1, gamma,
@@ -582,15 +613,46 @@ int launch_pair(const cfmm_bucket* b, int n_tokens, const double* nu, double eps
     return check_launch();
 }
 
+// StableSwap buckets: the LDG path only (the kernel is compute-bound; there is no TMA-staged variant)
+template <bool TRADES, bool HESS>
+int launch_stable(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                  const cfmm_eval_out* out, cudaStream_t st) {
+    const long long m = b->n_pools;
+    double* delta = out ? out->delta : nullptr;
+    double* lambda = out ? out->lambda : nullptr;
+    double* hcoef = out ? out->hcoef : nullptr;
+    if (use_shared(n_tokens, m)) {
+        const size_t sm = (size_t)n_tokens * sizeof(double);
+        auto kern = k_eval_stable<SharedScatter, TRADES, HESS>;
+        allow_smem(kern, sm);
+        kern<<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights,
+                                                    b->logrw, nu, psi, arb, delta, lambda, hcoef);
+    } else {
+        k_eval_stable<GlobalScatter, TRADES, HESS><<<grid_for(m, 8), kThreads, 0, st>>>(
+            m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights, b->logrw, nu, psi, arb, delta, lambda,
+            hcoef);
+    }
+    return check_launch();
+}
+
+template <int KIND, bool TRADES, bool HESS>
+int launch_kind(const cfmm_bucket* b, int n_tokens, const double* nu, double eps, double* psi, double* arb,
+                const cfmm_eval_out* out, cudaStream_t st) {
+    if constexpr (KIND == CFMM_KIND_STABLESWAP)
+        return launch_stable<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
+    else
+        return launch_pair<KIND, TRADES, HESS>(b, n_tokens, nu, eps, psi, arb, out, st);
+}
+
 template <int KIND>
 int dispatch_pair(const cfmm_bucket* b, int n_tokens, const double* nu, double eps, double* psi, double* arb,
                   const cfmm_eval_out* out, cudaStream_t st) {
     const bool trades = out && out->delta && out->lambda;
     const bool hess = out && out->hcoef;
-    if (trades && hess) return launch_pair<KIND, true, true>(b, n_tokens, nu, eps, psi, arb, out, st);
-    if (trades) return launch_pair<KIND, true, false>(b, n_tokens, nu, eps, psi, arb, out, st);
-    if (hess) return launch_pair<KIND, false, true>(b, n_tokens, nu, eps, psi, arb, out, st);
-    return launch_pair<KIND, false, false>(b, n_tokens, nu, eps, psi, arb, out, st);
+    if (trades && hess) return launch_kind<KIND, true, true>(b, n_tokens, nu, eps, psi, arb, out, st);
+    if (trades) return launch_kind<KIND, true, false>(b, n_tokens, nu, eps, psi, arb, out, st);
+    if (hess) return launch_kind<KIND, false, true>(b, n_tokens, nu, eps, psi, arb, out, st);
+    return launch_kind<KIND, false, false>(b, n_tokens, nu, eps, psi, arb, out, st);
 }
 
 template <int K, bool TRADES, bool HESS>
@@ -644,6 +706,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 2) return CFMM_E_KIND;
             if (b->n_pools > 0 && !b->weights) return CFMM_E_NULL;       // the offsets
             break;
+        case CFMM_KIND_STABLESWAP:
+            if (b->arity != 2) return CFMM_E_KIND;
+            if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // rates; (A, D)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -671,6 +737,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_SUM>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_BOUNDED_PRODUCT:
             return dispatch_pair<CFMM_KIND_BOUNDED_PRODUCT>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_STABLESWAP:
+            return dispatch_pair<CFMM_KIND_STABLESWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
         default:
             break;
     }

@@ -17,10 +17,10 @@ constexpr int kSmallThreads = 32;     // one warp per CTA: a sweep of 50 problem
 // LANES = 1: one problem per thread (throughput: 10^5 .. 10^6 problems).  LANES = 32: one problem per warp, the pool
 // loop of every evaluation split over the lanes (latency: a handful of problems, or problems with hundreds of pools);
 // each lane keeps its own copy of the state at work[(p * LANES + lane)], so `stride` counts lanes, not problems.
-template <int LANES>
-__global__ void __launch_bounds__(kSmallThreads)
-k_batch_solve(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm, int n, long long n_pools, double* work,
-              long long stride) {
+// STABLE: also evaluate StableSwap pools (k_batch_solve_stable); without it such a pool makes its problem status 3.
+template <int LANES, bool STABLE>
+__device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, const cfmm_batch& B, const cfmm_small::Params& prm,
+                                                 int n, long long n_pools, double* work, long long stride) {
     const long long gt = (long long)blockIdx.x * kSmallThreads + threadIdx.x;
     const long long p = LANES == 1 ? gt : gt / LANES;
     const int lane = LANES == 1 ? 0 : (int)(gt % LANES);
@@ -43,12 +43,28 @@ k_batch_solve(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm, int n, 
     Q.flags = B.flags + p * n;
     Q.delta = B.delta ? B.delta + p * B.trade_stride : nullptr;
     Q.lam = B.lambda ? B.lambda + p * B.trade_stride : nullptr;
-    const cfmm_small::Stats r = cfmm_small::solve_one<LANES>(P, Q, prm, B.nu + p * n, B.psi + p * n,
-                                                             work + (LANES == 1 ? p : p * LANES + lane), stride, lane);
+    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE>(P, Q, prm, B.nu + p * n, B.psi + p * n,
+                                                                     work + (LANES == 1 ? p : p * LANES + lane), stride, lane);
     if (lane == 0) {
         st[0] = r.value; st[1] = r.dual; st[2] = r.gap; st[3] = r.infeas; st[4] = r.err;
         st[5] = (double)r.iters; st[6] = (double)r.evals; st[7] = (double)r.status;
     }
+}
+
+template <int LANES>
+__global__ void __launch_bounds__(kSmallThreads)
+k_batch_solve(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm, int n, long long n_pools, double* work,
+              long long stride) {
+    batch_solve_body<LANES, false>(P, B, prm, n, n_pools, work, stride);
+}
+
+// the same solve for pool sets that hold StableSwap pools: its own instance, so that the Newton loops of
+// cfmm_small::stableswap_pair do not raise k_batch_solve's register count for problems without them
+template <int LANES>
+__global__ void __launch_bounds__(kSmallThreads)
+k_batch_solve_stable(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm, int n, long long n_pools, double* work,
+                     long long stride) {
+    batch_solve_body<LANES, true>(P, B, prm, n, n_pools, work, stride);
 }
 
 int g_batch_lanes = 1;       // cfmm_set_batch_lanes: 1 | 32
@@ -70,8 +86,9 @@ extern "C" int cfmm_set_batch_lanes(int32_t lanes) {
     return CFMM_OK;
 }
 
-extern "C" int cfmm_batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
-                                void* work, void* stream) {
+namespace {
+int batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm, void* work,
+                void* stream, bool stable) {
     if (!pools || !batch || !prm) return CFMM_E_NULL;
     if (batch->n_problems == 0) return CFMM_OK;
     if (!pools->pool_ptr || !pools->tok_idx || !pools->reserves || !pools->weights || !pools->logrw || !pools->gamma ||
@@ -84,11 +101,32 @@ extern "C" int cfmm_batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* b
                         pools->kind};
     cfmm_small::Params q{prm->tol, prm->eps0, prm->eps_min, prm->eps_shrink, prm->floor_rel, prm->max_outer, prm->max_inner};
     const long long stride = padded(batch->n_problems) * g_batch_lanes;      // state slots = CUDA threads
-    if (g_batch_lanes == 32)
-        k_batch_solve<32><<<(unsigned)(stride / kSmallThreads), kSmallThreads, 0, (cudaStream_t)stream>>>(
-            P, *batch, q, pools->n_tokens, pools->n_pools, (double*)work, stride);
-    else
-        k_batch_solve<1><<<(unsigned)(stride / kSmallThreads), kSmallThreads, 0, (cudaStream_t)stream>>>(
-            P, *batch, q, pools->n_tokens, pools->n_pools, (double*)work, stride);
+    const unsigned grid = (unsigned)(stride / kSmallThreads);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (stable) {
+        if (g_batch_lanes == 32)
+            k_batch_solve_stable<32><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools,
+                                                                     (double*)work, stride);
+        else
+            k_batch_solve_stable<1><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools,
+                                                                    (double*)work, stride);
+    } else if (g_batch_lanes == 32) {
+        k_batch_solve<32><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools, (double*)work,
+                                                          stride);
+    } else {
+        k_batch_solve<1><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools, (double*)work,
+                                                         stride);
+    }
     return check_launch();
+}
+}  // namespace
+
+extern "C" int cfmm_batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
+                                void* work, void* stream) {
+    return batch_solve(pools, batch, prm, work, stream, false);
+}
+
+extern "C" int cfmm_batch_solve_stableswap(const cfmm_csr_pools* pools, const cfmm_batch* batch,
+                                           const cfmm_batch_params* prm, void* work, void* stream) {
+    return batch_solve(pools, batch, prm, work, stream, true);
 }

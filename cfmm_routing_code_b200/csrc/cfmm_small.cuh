@@ -33,10 +33,12 @@ struct Pools {                       // CSR problem data (device pointers in the
     const int64_t* pool_ptr;         // [m+1]
     const int32_t* tok;              // [nnz]   token of every slot            arbitrage.py:6-12
     const double* R;                 // [nnz]   reserves                       arbitrage.py:14-20
-    const double* w;                 // [nnz]   normalised weights | 0 on constant-sum pools | virtual offsets (kind 3)
-    const double* logrw;             // [nnz]   log(R/w)
+    const double* w;                 // [nnz]   normalised weights | 0 on constant-sum pools | virtual offsets (kind 3) |
+                                     //         rates (kind 4)
+    const double* logrw;             // [nnz]   log(R/w) | kind 4: A at the pool's first slot, its invariant D at the second
     const double* gamma;             // [m]     fees                           arbitrage.py:22-28
-    const uint8_t* kind;             // [m]     1 = constant sum; 3 = bounded-liquidity product; 0 or 2 = weighted geometric mean
+    const uint8_t* kind;             // [m]     1 = constant sum; 3 = bounded-liquidity product; 4 = two-coin StableSwap;
+                                     //         0 or 2 = weighted geometric mean
                                      //         (constant product = equal weights)
 };
 
@@ -97,6 +99,90 @@ CFMM_HD inline void bounded_pair(double R0, double R1, double o0, double o1, dou
     }
 }
 
+// Two-coin StableSwap (Curve) pool: scaled balances y_j = r_j x_j on the invariant
+//     4A (y0 + y1) + D = 4A D + D^3 / (4 y0 y1),        D = the invariant of the current reserves (precomputed),
+// worked in units of D (u_j = y_j / D, so 4A (u0 + u1) + 1 = 4A + 1 / (4 u0 u1)) so nothing overflows.  Along the curve
+// the marginal rate -du_b/du_a is s = F_a / F_b, F_a = 4A + G / u_a, F_b = 4A + G / u_b, G = 1 / (4 u_a u_b); in token
+// units p = (r_a / r_b) s.  Tendering a pays iff gamma nu_b p(R) > nu_a; the optimal post-trade balance solves
+// s(u_a) = q* = mu_a / (gamma mu_b) with the scaled prices mu_j = nu_j / r_j, found by a safeguarded Newton iteration on
+// t = log u_a (s falls from +inf to 0 along the curve, so an upper bracket always exists).  u_b(u_a) is Curve's get_y:
+// the positive root of u^2 + b u - c with b = u_a + 1/(4A) - 1, c = 1 / (16 A u_a), in the cancellation-free form.
+// hc = nu_0 dy_0/dlog nu_0 = -nu_a X_a / (gamma dlog s/dt) at the solution (0 without a trade).
+// Fixed iteration caps and a deterministic exit; shared by the per-thread solver and k_eval_stable (cfmm_kernels.cu).
+CFMM_HD inline double stableswap_get_y(double ua, double A) {
+    const double b = (ua - 1.0) + 0.25 / A, c = 0.0625 / (A * ua);
+    const double sq = sqrt(b * b + 4.0 * c);
+    return b > 0.0 ? 2.0 * c / (b + sq) : 0.5 * (sq - b);
+}
+
+// log s - logq at u_a = exp(t) on the curve, and its derivative in t
+CFMM_HD inline double stableswap_phi(double t, double A, double logq, double* dphi) {
+    const double ua = exp(t), ub = stableswap_get_y(ua, A);
+    const double G = 0.25 / (ua * ub);
+    const double Fa = 4.0 * A + G / ua, Fb = 4.0 * A + G / ub;
+    const double kap = -(Fa / Fb) * (ua / ub);                          // dlog u_b / dlog u_a along the curve
+    *dphi = (G / ua) * (-2.0 - kap) / Fa - (G / ub) * (-1.0 - 2.0 * kap) / Fb;
+    // s = 1 + del, del = (F_a - F_b) / F_b without cancellation: log1p near s = 1, the plain ratio far from it
+    const double del = G * (ub - ua) / (ua * ub * Fb);
+    return (fabs(del) < 0.5 ? log1p(del) : log(Fa / Fb)) - logq;
+}
+
+// One direction of stableswap_pair: tender a, receive b.  Balances in units of D (ua, ub), scaled prices mu = nu / r.
+// Writes the tender Delta_a and the payout Lambda_b and returns hc (all 0 without a trade).  Scalar arguments only: the
+// two calls below take the directions with constant operands, so nothing is indexed by a loop variable (no stack).
+CFMM_HD inline double stableswap_dir(double Ra, double Rb, double ra, double rb, double ua0, double ub0, double mua,
+                                     double mub, double nua, double A, double Dinv, double gam, double& Da, double& Lb) {
+    Da = Lb = 0.0;
+    const double G0 = 0.25 / (ua0 * ub0);
+    const double Fa = 4.0 * A + G0 / ua0, Fb = 4.0 * A + G0 / ub0;
+    const double del = G0 * (ub0 - ua0) / (ua0 * ub0 * Fb);
+    const double s0 = fabs(del) < 0.5 ? 1.0 + del : Fa / Fb;            // the marginal rate at R, as in stableswap_phi
+    if (!(gam * mub * s0 > mua)) return 0.0;                            // no trade in this direction
+    const double logq = log(mua / (gam * mub));
+    double lo = log(ua0), hi = lo, dphi = 0.0;
+    for (double step = 1.0; step <= 512.0; step *= 2.0) {               // upper bracket phi(hi) <= 0 (|t| < 700: exp finite)
+        hi = lo + step;
+        if (!(stableswap_phi(hi, A, logq, &dphi) > 0.0)) break;
+        lo = hi;
+    }
+    // safeguarded Newton inside [lo, hi]: a bisection step whenever the Newton step would leave the bracket or would
+    // not at least halve the step before last (a crawl where phi bends), so the bracket keeps shrinking
+    double t = lo, dx_old = hi - lo, dx = dx_old;
+    for (int it = 0; it < 100; ++it) {
+        const double f = stableswap_phi(t, A, logq, &dphi);
+        if (f > 0.0) lo = t; else hi = t;
+        if (f == 0.0 || !(hi - lo > 4e-16 * (1.0 + fabs(t)))) break;
+        const double tn = t - f / dphi;
+        // phi is at the level of its own rounding (a few u of log s, u |log q*|): further steps would only chase that
+        // noise (a flat curve, large A, |phi'| small); the last Newton step, inside the bracket, is as good as any
+        if (fabs(f) <= 8e-16 * (1.0 + fabs(logq))) {
+            if (tn > lo && tn < hi) t = tn;
+            break;
+        }
+        if (!(tn > lo && tn < hi) || fabs(2.0 * f) > fabs(dx_old * dphi)) {
+            dx_old = dx; dx = 0.5 * (hi - lo); t = lo + dx;
+        } else {
+            dx_old = dx; dx = tn - t; t = tn;
+        }
+        if (fabs(dx) <= 1e-15 * (1.0 + fabs(t))) break;
+    }
+    const double ua = exp(t), ub = stableswap_get_y(ua, A);
+    const double Xa = fmax(ua * Dinv / ra, Ra), Xb = ub * Dinv / rb;
+    Da = (Xa - Ra) / gam;
+    Lb = fmax(Rb - Xb, 0.0);
+    stableswap_phi(t, A, logq, &dphi);
+    return dphi < 0.0 ? -nua * Xa / (gam * dphi) : 0.0;
+}
+
+CFMM_HD inline void stableswap_pair(double R0, double R1, double r0, double r1, double A, double Dinv, double gam,
+                                    double n0, double n1, double* D, double* L, double& hc) {
+    const double u0 = r0 * R0 / Dinv, u1 = r1 * R1 / Dinv, mu0 = n0 / r0, mu1 = n1 / r1;
+    double d0, l1, d1, l0;
+    hc = stableswap_dir(R0, R1, r0, r1, u0, u1, mu0, mu1, n0, A, Dinv, gam, d0, l1)
+       + stableswap_dir(R1, R0, r1, r0, u1, u0, mu1, mu0, n1, A, Dinv, gam, d1, l0);
+    D[0] = d0; D[1] = d1; L[0] = l0; L[1] = l1;
+}
+
 #ifdef __CUDA_ARCH__
 // sum over the LANES consecutive lanes that share a problem; x + y == y + x exactly, so every lane ends with the same bits
 template <int LANES>
@@ -114,7 +200,9 @@ __device__ __forceinline__ double lanes_sum(double v) {
 // state and runs the identical instruction stream; only this pool loop is split (lane l takes pools l, l+LANES, ...)
 // and the partial psi / arb / Hessian / fills are then summed over the lanes with an xor butterfly, which leaves
 // bit-identical totals in every lane -- so the lanes never diverge and need no other communication.
-template <int LANES>
+// STABLE: the instance that also evaluates StableSwap pools (kind 4).  The plain instance keeps the register budget it
+// had before that kind existed and rejects such pools (solve_one: status 3); cfmm_batch_solve_stableswap runs the other.
+template <int LANES, bool STABLE = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane) {
     const int n = Q.n;
@@ -130,9 +218,13 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
         const int k = (int)(P.pool_ptr[i + 1] - off);
         const double gam = P.gamma[i];
         double D[KMAX], L[KMAX];
-        if (P.kind[i] == 3) {
+        if (P.kind[i] == 3 || (STABLE && P.kind[i] == 4)) {
             double hc = 0.0;
-            bounded_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], gam, nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
+            if (!STABLE || P.kind[i] == 3)
+                bounded_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], gam, nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
+            else                                                           // rates in w, (A, D) in logrw
+                stableswap_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], P.logrw[off], P.logrw[off + 1], gam,
+                                nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
             if (Hs && hc != 0.0) {
                 const int t0 = P.tok[off], t1 = P.tok[off + 1];
                 (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
@@ -324,7 +416,7 @@ CFMM_HD inline int newton_direction(int n, uint64_t free_mask, const Vec& Hs, co
 CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL * n * n + (int64_t)n * (n + 1) + 2 * nnz; }
 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
-template <int LANES = 1>
+template <int LANES = 1, bool STABLE = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0) {
     const int n = Q.n;
@@ -344,7 +436,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int64_t o = P.pool_ptr[i];
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1;
-        bad = P.kind[i] > 3 || k < 2 || k > KMAX || ((P.kind[i] == 1 || P.kind[i] == 3) && k != 2);
+        bad = P.kind[i] > (STABLE ? 4 : 3) || k < 2 || k > KMAX ||
+              ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && P.kind[i] == 4)) && k != 2);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
     if (bad) {
@@ -371,7 +464,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -417,7 +510,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -442,8 +535,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
+        evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -468,8 +561,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
+    evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

@@ -133,6 +133,59 @@ def synth_mixed(m, n_tokens, seed, frac_product=0.6, frac_weighted=0.3, misprici
     )
 
 
+def synth_stable_market(m, n_tokens, seed, frac_stable=0.3, frac_weighted=0.1, n_stable=8, mispricing=0.02):
+    """A market with a stablecoin cluster: tokens 0..n_stable-1 trade near 1 (within +-0.2 %), the last three of them
+    are rate-bearing (worth 1.02 / 1.05 / 1.1 of the others: wrapped or yield-bearing stablecoins).  StableSwap pools
+    (A in {50 .. 2000}, Curve's usual range; rates = the tokens' values) join pairs of the cluster, beside constant-
+    product pools over all tokens (the cluster included) and weighted pools of arity 2..4.  Balances are imbalanced by
+    up to ~2x and mispriced by `mispricing`.  Returns CSR arrays (HostPools(**out) minus `prices`) plus the prices."""
+    rng = np.random.default_rng(seed)
+    n_stable = min(n_stable, n_tokens)
+    p = np.exp(rng.standard_normal(n_tokens))
+    rate = np.ones(n_tokens)
+    rate[max(0, n_stable - 3):n_stable] = [1.02, 1.05, 1.1][-min(3, n_stable):]
+    p[:n_stable] = rate[:n_stable] * np.exp(0.002 * rng.uniform(-1, 1, n_stable))
+    n_ss = int(round(frac_stable * m)) if n_stable >= 2 else 0
+    n_w = int(round(frac_weighted * m)); n_cp = m - n_ss - n_w
+    # constant product over all tokens
+    a = rng.integers(0, n_tokens, n_cp); b = (a + rng.integers(1, n_tokens, n_cp)) % n_tokens
+    liq = np.exp(8.0 + 1.5 * rng.standard_normal(n_cp))
+    out_idx = [np.stack([a, b], 1)]
+    out_R = [np.stack([liq / p[a], liq / p[b]], 1) * np.exp(mispricing * rng.standard_normal((n_cp, 2)))]
+    out_w = [np.full((n_cp, 2), 0.5)]; out_g = [_FEES[rng.integers(0, 3, n_cp)]]; out_k = [np.zeros(n_cp, np.uint8)]
+    out_ar = [np.full(n_cp, 2)]; out_amp = [np.zeros(n_cp)]
+    # weighted pools
+    for k in (2, 3, 4):
+        mk = n_w // 3 + (1 if k - 2 < n_w % 3 else 0)
+        if mk == 0 or k > n_tokens:
+            continue
+        toks = np.stack([rng.choice(n_tokens, k, replace=False) for _ in range(mk)])
+        w = rng.dirichlet(np.ones(k), mk); w = np.maximum(w, 0.05); w /= w.sum(1, keepdims=True)
+        L = np.exp(8.0 + 1.5 * rng.standard_normal(mk))
+        out_idx.append(toks); out_R.append(L[:, None] * w / p[toks] * np.exp(mispricing * rng.standard_normal((mk, k))))
+        out_w.append(w); out_g.append(_FEES[rng.integers(0, 3, mk)]); out_k.append(np.zeros(mk, np.uint8))
+        out_ar.append(np.full(mk, k)); out_amp.append(np.zeros(mk))
+    # StableSwap pools inside the cluster: value-balanced up to a factor ~2, rates = the tokens' values
+    if n_ss:
+        sa = rng.integers(0, n_stable, n_ss); sb = (sa + rng.integers(1, n_stable, n_ss)) % n_stable
+        V = np.exp(9.0 + 1.5 * rng.standard_normal(n_ss))
+        imb = np.exp(0.35 * rng.standard_normal(n_ss))
+        R = np.stack([V * imb / p[sa], V / imb / p[sb]], 1) * np.exp(mispricing * rng.standard_normal((n_ss, 2)))
+        out_idx.append(np.stack([sa, sb], 1)); out_R.append(R); out_w.append(np.stack([rate[sa], rate[sb]], 1))
+        out_g.append(np.array([0.9996, 0.9999, 0.99995])[rng.integers(0, 3, n_ss)])
+        out_k.append(np.full(n_ss, 4, np.uint8)); out_ar.append(np.full(n_ss, 2))
+        out_amp.append(np.array([50.0, 100.0, 200.0, 1000.0, 2000.0])[rng.integers(0, 5, n_ss)])
+    arity = np.concatenate(out_ar)
+    return dict(
+        n_tokens=n_tokens, prices=p,
+        pool_ptr=np.concatenate([[0], np.cumsum(arity)]).astype(np.int64),
+        tok_idx=np.concatenate([x.ravel() for x in out_idx]).astype(np.int32),
+        reserves=np.concatenate([x.ravel() for x in out_R]),
+        weights=np.concatenate([x.ravel() for x in out_w]),
+        gamma=np.concatenate(out_g), kind=np.concatenate(out_k), amp=np.concatenate(out_amp),
+    )
+
+
 def synth_basket(n_tokens, prices, seed, n_assets=16, scale=1e-3, liq_mean=np.exp(8.0)):
     """cfg 4 basket: a_j = exp(N(0,1)) * Lbar / p_j * 1e-3 on 16 random tokens, target token 0."""
     rng = np.random.default_rng(seed)

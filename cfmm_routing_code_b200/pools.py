@@ -19,6 +19,34 @@ from . import _lib
 KIND_GEOMEAN_HOST = 0   # host CSR convention: 0 = (weighted) geometric mean, 1 = constant sum
 KIND_SUM_HOST = 1
 KIND_BOUNDED_HOST = 3   # constant product on virtual reserves (reserves + offsets), real reserves >= 0; offsets ride in `weights`
+KIND_STABLESWAP_HOST = 4  # two-coin StableSwap (Curve); rates ride in `weights`, the amplification in HostPools.amp
+AMP_MAX = 1e7           # largest StableSwap amplification A accepted
+
+
+def stableswap_invariant(reserves, rates, amp) -> np.ndarray:
+    """Invariant D of two-coin StableSwap pools: the root of 4A (y0 + y1) + D = 4A D + D^3 / (4 y0 y1) with the scaled
+    balances y = rates * reserves.  reserves, rates: (m, 2); amp: (m,) (Curve's A(), not A n^n).  Curve's get_D Newton
+    iteration in fp64 on the balances in units of y0 + y1 (the invariant is homogeneous of degree 1), from D = y0 + y1
+    down to the root (monotone: the cubic is convex there); a pool stops once a step
+    moves D by at most 2 ulp.  Elementwise: a pool's D does not depend on the other pools of the call, so a subset
+    (PoolStore.update_pools) gives the same bits as the whole."""
+    y = np.asarray(reserves, np.float64).reshape(-1, 2) * np.asarray(rates, np.float64).reshape(-1, 2)
+    A = np.asarray(amp, np.float64).reshape(-1)
+    scale = y[:, 0] + y[:, 1]
+    with np.errstate(all="ignore"):
+        y0, y1 = y[:, 0] / scale, y[:, 1] / scale                         # units of y0 + y1: nothing over- or underflows
+        S = y0 + y1
+        out = S.copy()
+        act = np.arange(len(S))
+        for _ in range(255):
+            if len(act) == 0:
+                break
+            d, ann = out[act], 4.0 * A[act]
+            dp = d * d / (2.0 * y0[act]) * d / (2.0 * y1[act])               # D^3 / (4 y0 y1)
+            dn = (ann * S[act] + 2.0 * dp) * d / ((ann - 1.0) * d + 3.0 * dp)
+            out[act] = dn
+            act = act[~(np.abs(dn - d) <= 4.5e-16 * dn)]
+    return out * scale
 
 
 @dataclasses.dataclass
@@ -28,9 +56,22 @@ class HostPools:
     pool_ptr: np.ndarray   # int64 [m+1]
     tok_idx: np.ndarray    # int32 [nnz]
     reserves: np.ndarray   # f64 [nnz]
-    weights: np.ndarray    # f64 [nnz]  normalised per pool; ignored for constant-sum
+    weights: np.ndarray    # f64 [nnz]  normalised per pool; ignored for constant-sum; rates of StableSwap pools
     gamma: np.ndarray      # f64 [m]
     kind: np.ndarray       # uint8 [m]
+    amp: Optional[np.ndarray] = None   # f64 [m]  StableSwap amplification A, 0 on other kinds (None: all zero)
+    inv: Optional[np.ndarray] = None   # f64 [m]  StableSwap invariant D of the reserves, 0 on other kinds (None: computed)
+
+    def __post_init__(self):
+        m = len(self.gamma)
+        if self.amp is None:
+            self.amp = np.zeros(m)
+        if self.inv is None:
+            self.inv = np.zeros(m)
+            ss = np.nonzero(np.asarray(self.kind) == KIND_STABLESWAP_HOST)[0]
+            if len(ss):
+                off = np.asarray(self.pool_ptr)[ss][:, None] + np.arange(2)
+                self.inv[ss] = stableswap_invariant(self.reserves[off], self.weights[off], self.amp[ss])
 
     @property
     def m(self) -> int:
@@ -40,11 +81,14 @@ class HostPools:
     def from_lists(n_tokens, local_indices, reserves, fees, kinds, weights=None) -> "HostPools":
         """From the reference's literals: local_indices / reserves / fees (arbitrage.py:6-28) plus
         which cvxpy atom constrains each pool (arbitrage.py:63-74): 'geomean' (with weights[i] = the
-        ``p=`` vector), 'product' (cp.geo_mean on 2 tokens) or 'sum'."""
+        ``p=`` vector), 'product' (cp.geo_mean on 2 tokens) or 'sum'.  Beyond the reference: 'bounded_product' (weights[i]
+        = the two virtual-reserve offsets) and 'stableswap' (weights[i] = (A, r0, r1): Curve's amplification A() and
+        rate multipliers, (A, 1, 1) for a plain pool)."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
         ptr = [0]; idx: List[int] = []; res: List[float] = []; wts: List[float] = []; kd: List[int] = []
+        amp = np.zeros(m)
         for i, l in enumerate(local_indices):
             k = len(l)
             if len(reserves[i]) != k:
@@ -64,6 +108,12 @@ class HostPools:
                 if k != 2 or o is None or len(o) != 2 or np.any(o < 0) or not np.all(np.isfinite(o)):
                     raise ValueError(f"pool {i}: bounded_product needs 2 tokens and 2 non-negative offsets in weights[i]")
                 kd.append(KIND_BOUNDED_HOST); wts += list(o)
+            elif kinds[i] == "stableswap":
+                p = None if (weights is None or weights[i] is None) else np.asarray(weights[i], float).reshape(-1)
+                if k != 2 or p is None or len(p) != 3:
+                    raise ValueError(f"pool {i}: stableswap needs 2 tokens and weights[i] = (A, r0, r1)")
+                _check_stableswap(p[0], p[1:], reserves[i], f"pool {i}: ")
+                kd.append(KIND_STABLESWAP_HOST); wts += [float(p[1]), float(p[2])]; amp[i] = p[0]
             elif kinds[i] in ("geomean", "product"):
                 w = np.ones(k) if (weights is None or weights[i] is None) else np.asarray(weights[i], float)
                 if len(w) != k or np.any(w <= 0):
@@ -73,7 +123,7 @@ class HostPools:
                 raise ValueError(f"pool {i}: unknown kind {kinds[i]!r}")
         return HostPools(int(n_tokens), np.asarray(ptr, np.int64), np.asarray(idx, np.int32),
                          np.asarray(res, np.float64), np.asarray(wts, np.float64),
-                         np.asarray(fees, np.float64), np.asarray(kd, np.uint8))
+                         np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp)
 
     @staticmethod
     def from_pairs(n_tokens, idx, reserves, gamma) -> "HostPools":
@@ -106,6 +156,26 @@ class HostPools:
             raise ValueError("fees (gamma) must lie in (0, 1]")
         if self.tok_idx.min(initial=0) < 0 or self.tok_idx.max(initial=0) >= self.n_tokens:
             raise ValueError("token index out of range")
+        ss = np.nonzero(np.asarray(self.kind) == KIND_STABLESWAP_HOST)[0]
+        if len(ss):
+            if np.any(np.diff(self.pool_ptr)[ss] != 2):
+                raise ValueError("stableswap pools must have 2 tokens")
+            off = self.pool_ptr[ss][:, None] + np.arange(2)
+            _check_stableswap(self.amp[ss], self.weights[off], self.reserves[off])
+            D = np.asarray(self.inv, float)[ss]
+            if not bool(np.all(np.isfinite(D) & (D > 0))):
+                raise ValueError("stableswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
+
+
+def _check_stableswap(A, rates, reserves, where=""):
+    """The value rules of StableSwap pools: A finite in (0, AMP_MAX], rates finite and > 0, reserves finite and > 0."""
+    A, r, R = np.asarray(A, float), np.asarray(rates, float), np.asarray(reserves, float)
+    if not bool(np.all((A > 0) & (A <= AMP_MAX))):
+        raise ValueError(f"{where}stableswap amplification A must be finite and in (0, {AMP_MAX:g}]")
+    if not bool(np.all(np.isfinite(r) & (r > 0))):
+        raise ValueError(f"{where}stableswap rates must be finite and > 0")
+    if not bool(np.all(np.isfinite(R) & (R > 0))):
+        raise ValueError(f"{where}stableswap reserves must be finite and > 0")
 
 
 @dataclasses.dataclass
@@ -245,6 +315,11 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         if np.any(ar[bp] != 2):
             raise ValueError("bounded_product pools must have 2 tokens")
         keys.append((_lib.KIND_BOUNDED, 2, np.nonzero(bp)[0]))
+    ss = hp.kind == KIND_STABLESWAP_HOST
+    if ss.any():
+        if np.any(ar[ss] != 2):
+            raise ValueError("stableswap pools must have 2 tokens")
+        keys.append((_lib.KIND_STABLESWAP, 2, np.nonzero(ss)[0]))
     gm = (hp.kind == KIND_GEOMEAN_HOST) & ~is_cp
     for k in np.unique(ar[gm]).tolist():
         if k < 2 or k > 32:
@@ -299,6 +374,10 @@ class DeviceBucket:
             self.logrw = torch.as_tensor(_padded(np.log(R / W), self.stride, 0.0), **f64)
         if self.kind == _lib.KIND_BOUNDED:                 # the virtual-reserve offsets ride in the weights slot
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
+        if self.kind == _lib.KIND_STABLESWAP:              # rates in the weights slot, (A, D) in the two logrw slots
+            self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
+            AD = np.stack([hp.amp[spec.sel], hp.inv[spec.sel]])
+            self.logrw = torch.as_tensor(_padded(AD, self.stride, 1.0), **f64)
         if self.kind == _lib.KIND_SUM:
             self.theta_bar = torch.zeros((2, self.stride), **f64)
         self.delta = self.lam = self.hcoef = self.hmask = None
@@ -319,14 +398,17 @@ class DeviceBucket:
         return self.spec.off
 
     def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
-                     W: Optional[np.ndarray] = None):
+                     W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None):
         """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
-        Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__."""
+        Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__;
+        StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,)."""
         f64 = dict(dtype=torch.float64, device=self._device)
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
         if R is not None:
             self.reserves[:, li] = torch.as_tensor(R, **f64)
-            if self.logrw is not None:
+            if self.kind == _lib.KIND_STABLESWAP:
+                self.logrw[1, li] = torch.as_tensor(stableswap_invariant(R.T, W.T, amp), **f64)
+            elif self.logrw is not None:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
         if gamma is not None:
             self.gamma[li] = torch.as_tensor(gamma, **f64)
@@ -768,7 +850,8 @@ class PoolStore:
         self.m_total = hp.m
         self.pool_ptr = hp.pool_ptr
         self._tok_idx_host = hp.tok_idx
-        self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets
+        self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets / rates
+        self._amp_host = hp.amp                                          # StableSwap amplification (structure too)
         self._where = None                                               # pool -> (bucket, position): update_pools
         self.rank, self.world = rank, world
         self.buckets = []
@@ -829,7 +912,8 @@ class PoolStore:
         """SURVEY.md section 8(d): 32 B per 2-token pool, 28k+12 per weighted pool, + nu, psi, arb."""
         n = 0
         for b in self.buckets:
-            n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED else 32)
+            n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED
+                        else 64 if b.kind == _lib.KIND_STABLESWAP else 32)
         return n + 16 * self.n_tokens + 8
 
     # -- the hot path --------------------------------------------------------------------------
@@ -943,7 +1027,9 @@ class PoolStore:
         from the updated host data, without re-uploading the pools or rebuilding the blocked layout (which depends on the
         token ids only).  pool_ids: global pool indices (the order of the problem's local_indices); reserves[k]: the new
         reserve vector of pool pool_ids[k], with the pool's arity (an (n, 2) array for pairs); fees[k]: its new gamma in
-        (0, 1].  At least one of reserves / fees.  Kinds, tokens, weights and bounded_product offsets cannot change.
+        (0, 1].  At least one of reserves / fees.  Kinds, tokens, weights, bounded_product offsets and StableSwap
+        amplifications and rates cannot change (they are structure: build a new store, e.g. for a ramp of A); a StableSwap
+        pool's invariant D is recomputed from its new reserves, as HostPools does.
 
         All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.validate) raise
         ValueError before anything is written, and so does an entry the device check of the blocked bucket rejects.
@@ -965,16 +1051,17 @@ class PoolStore:
             rs = u.ptr[e][None, :] + np.arange(b.arity)[:, None]          # (arity, n) indices into the update's slots
             R = None if u.reserves is None else u.reserves[rs]
             g = None if u.gamma is None else u.gamma[e]
-            plan.append((b, loc[u.ids[e]], R, g, rs))
+            plan.append((b, loc[u.ids[e]], R, g, rs, u.ids[e]))
         # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
         rebuilt = 0
-        for b, l, R, g, _ in plan:
+        for b, l, R, g, _, _ in plan:
             if getattr(b, "blocked", False):
                 rebuilt += b.write_update(self.lib, l, R, g, self._stream())
-        for b, l, R, g, rs in plan:
+        for b, l, R, g, rs, ids in plan:
             if not getattr(b, "blocked", False):
                 W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None) else None
-                b.write_update(l, R, g, W)
+                amp = self._amp_host[ids] if b.kind == _lib.KIND_STABLESWAP else None
+                b.write_update(l, R, g, W, amp)
         torch.cuda.synchronize(self.device)
         return rebuilt
 

@@ -13,7 +13,8 @@
  *   tok_idx [k][n_pools]  i32   local_indices  arbitrage.py:6-12   (replaces dense A_i, :42-48)
  *   gamma   [n_pools]     f64   fees[i]        arbitrage.py:22-28
  *   weights [k][n_pools]  f64   normalised p/sum(p) of cp.geo_mean(x, p=...)   arbitrage.py:65
- *   logrw   [k][n_pools]  f64   log(R/w), precomputed once (weighted pools only)
+ *   logrw   [k][n_pools]  f64   log(R/w), precomputed once (weighted pools); StableSwap: (A, D) per pool
+ *   (StableSwap pools carry their rates in `weights`, bounded products their virtual-reserve offsets)
  *   theta_bar[2][n_pools] f64   constant-sum fills (multipliers of the kink), updated by the solver
  */
 #ifndef CFMM_B200_H
@@ -29,9 +30,13 @@ enum {
     CFMM_KIND_PRODUCT = 0, /* sqrt(x1 x2) >= sqrt(R1 R2)                 arbitrage.py:68-70 */
     CFMM_KIND_SUM = 1,     /* sum(x) >= sum(R), x >= 0                   arbitrage.py:73-74 */
     CFMM_KIND_GEOMEAN = 2, /* prod x^w >= prod R^w                       arbitrage.py:65    */
-    CFMM_KIND_BOUNDED_PRODUCT = 3 /* sqrt((x1+o1)(x2+o2)) >= sqrt((R1+o1)(R2+o2)), x >= 0: constant product on virtual
+    CFMM_KIND_BOUNDED_PRODUCT = 3, /* sqrt((x1+o1)(x2+o2)) >= sqrt((R1+o1)(R2+o2)), x >= 0: constant product on virtual
                               reserves, one Uniswap-v3 tick range.  Not in the reference (a new atom for the cons list
                               of arbitrage.py:63-74); arity 2, the two offsets passed in `weights`                */
+    CFMM_KIND_STABLESWAP = 4 /* two-coin StableSwap (Curve): 4A(y0+y1) + D >= 4AD + D^3/(4 y0 y1), y_j = r_j x_j, where
+                              D = D(R) is the invariant of the current reserves.  Not in the reference; arity 2.
+                              weights [2][stride] = the rates (r0, r1) > 0; logrw [2][stride] = per-pool constants:
+                              slot 0 = A (Curve's A(), not A n^n), slot 1 = D.  Smooth (no kink): no theta_bar       */
 };
 
 enum {
@@ -53,8 +58,8 @@ typedef struct cfmm_bucket {
     const double* reserves;
     const int32_t* tok_idx;
     const double* gamma;
-    const double* weights;   /* GEOMEAN only */
-    const double* logrw;     /* GEOMEAN only */
+    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP rates */
+    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP (A, D) */
     const double* theta_bar; /* SUM only     */
 } cfmm_bucket;
 
@@ -266,10 +271,13 @@ typedef struct cfmm_csr_pools {
     const int64_t* pool_ptr;   /* [n_pools+1]                                                        */
     const int32_t* tok_idx;    /* [nnz]  local_indices, arbitrage.py:6-12                             */
     const double* reserves;    /* [nnz]  arbitrage.py:14-20                                          */
-    const double* weights;     /* [nnz]  normalised like cp.geo_mean(p=...), arbitrage.py:65; 0 on constant-sum pools */
-    const double* logrw;       /* [nnz]  log(reserves / weights) (unused on constant-sum pools)      */
+    const double* weights;     /* [nnz]  normalised like cp.geo_mean(p=...), arbitrage.py:65; 0 on constant-sum pools;
+                                         offsets of bounded products; rates of StableSwap pools        */
+    const double* logrw;       /* [nnz]  log(reserves / weights) (unused on constant-sum pools); StableSwap: A at the
+                                         pool's first slot, D at its second                            */
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
-    const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT, else weighted geometric mean */
+    const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP, else
+                                            weighted geometric mean                                  */
 } cfmm_csr_pools;
 
 typedef struct cfmm_batch {
@@ -301,6 +309,11 @@ int64_t cfmm_batch_solve_work_bytes(const cfmm_csr_pools* pools, int32_t n_probl
 int cfmm_set_batch_lanes(int32_t lanes);
 int cfmm_batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm, void* work,
                      void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_STABLESWAP pools (cfmm_batch_solve gives their problems status 3).
+ * A separate kernel instance: the per-pool Newton solve of those pools needs more registers than the other kinds, and
+ * cfmm_batch_solve keeps the occupancy it has without them.  Same arguments, limits and workspace. */
+int cfmm_batch_solve_stableswap(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
+                                void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
