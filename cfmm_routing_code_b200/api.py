@@ -105,8 +105,8 @@ def solve(local_indices, reserves, fees, kinds, weights=None, utility=None, n_to
           **solver_kw) -> Result:
     """Solve the routing problem the reference scripts pose.  `kinds[i]` in {'geomean','product','sum'}
     names the cvxpy atom on pool i (arbitrage.py:63-74); `weights[i]` is the geo_mean ``p=`` vector.  Two more kinds:
-    'bounded_product' (weights[i] = virtual-reserve offsets) and 'stableswap' (weights[i] = (A, r0, r1), a two-coin
-    Curve pool; see HostPools.from_lists)."""
+    'bounded_product' (weights[i] = virtual-reserve offsets) and 'stableswap' (weights[i] = (A, r_0, ..., r_{n-1}), a
+    Curve pool of 2..8 coins with the whitepaper A = A() / n^(n-1); see HostPools.from_lists)."""
     if utility is None:
         raise ValueError("utility is required: Arbitrage(c) | Liquidate(target, assets) | Swap(i, o, t)")
     if n_tokens is None:

@@ -50,6 +50,8 @@ class CsrStore:
         self.logrw = torch.log(torch.clamp(self.R, min=1e-300) / torch.as_tensor(w, device=dev))
         ss = np.nonzero(np.asarray(hp.kind) == KIND_STABLESWAP_HOST)[0]
         self.has_stableswap = bool(len(ss))         # -> cfmm_batch_solve_stableswap (its own kernel instance)
+        # pools of more than two coins -> cfmm_batch_solve_stableswap_n (a third instance, which takes every arity)
+        self.has_stableswap_n = bool(len(ss)) and bool(np.any(np.diff(np.asarray(hp.pool_ptr))[ss] > 2))
         if len(ss):                                  # StableSwap pools: A at the first slot, the invariant D at the second
             first = torch.as_tensor(np.asarray(hp.pool_ptr)[ss], device=dev)
             self.logrw[first] = torch.as_tensor(np.asarray(hp.amp, np.float64)[ss], device=dev)
@@ -106,7 +108,8 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    entry = store.lib.cfmm_batch_solve_stableswap if store.has_stableswap else store.lib.cfmm_batch_solve
+    entry = (store.lib.cfmm_batch_solve_stableswap_n if store.has_stableswap_n else
+             store.lib.cfmm_batch_solve_stableswap if store.has_stableswap else store.lib.cfmm_batch_solve)
     _lib.check(entry(C.byref(store.c_pools), C.byref(batch), C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve")
     return psi, stats, delta, lam
 

@@ -206,6 +206,47 @@ k_eval_stable(long long m, long long ld, int n_tokens, const double* __restrict_
     block_accumulate(acc, arb);
 }
 
+// n-coin StableSwap, arity K (3..8; 2 for the cross-check against k_eval_stable): cfmm_small::stableswap_n (a
+// breakpoint root per step of a safeguarded Newton iteration, compute-bound), one thread per pool.  rates [K][ld] (the
+// bucket's weights), AD [2][ld] = (A, D) (the bucket's logrw).  hcoef [K][ld] = the per-slot h_j, hmask = traded slots.
+template <int K, typename Scatter, bool TRADES, bool HESS>
+__global__ void __launch_bounds__(kThreads)
+k_eval_stable_n(long long m, long long ld, int n_tokens, const double* __restrict__ R, const int* __restrict__ idx,
+                const double* __restrict__ gamma, const double* __restrict__ rates, const double* __restrict__ AD,
+                const double* __restrict__ nu, double* psi, double* arb, double* delta, double* lambda, double* hcoef,
+                uint32_t* hmask) {
+    extern __shared__ double smem[];
+    Scatter sc{psi};
+    sc.init(smem, n_tokens);
+    double acc = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        double Rl[K], rl[K], nl[K], D[K], L[K], h[K];
+        int id[K];
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+            id[j] = idx[(long long)j * ld + i];
+            Rl[j] = R[(long long)j * ld + i];
+            rl[j] = rates[(long long)j * ld + i];
+            nl[j] = __ldg(nu + id[j]);
+        }
+        const uint32_t mask = cfmm_small::stableswap_n<K>(K, Rl, rl, AD[i], AD[ld + i], gamma[i], nl, D, L, h);
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+            if (TRADES) { delta[(long long)j * ld + i] = D[j]; lambda[(long long)j * ld + i] = L[j]; }
+            if (HESS) hcoef[(long long)j * ld + i] = h[j];
+            const double y = L[j] - D[j];
+            if (y != 0.0) {
+                sc.add(id[j], y);
+                acc += nl[j] * y;
+            }
+        }
+        if (HESS) hmask[i] = mask;
+    }
+    sc.flush(smem, n_tokens);
+    block_accumulate(acc, arb);
+}
+
 // ---------------------------------------------------------------------------------------------
 // TMA-staged variant of the 2-token kernel: persistent CTAs, each walking tiles of kTile pools.
 // One elected thread issues five 1-D bulk copies per tile (cp.async.bulk -> UBLKCP: R0, R1, gamma,
@@ -410,6 +451,7 @@ k_eval_geomean(long long m, long long ld, int karity, int n_tokens, const double
 // Hessian-vector product / diagonal / dense assembly, log-price coordinates
 //   2-token kinds:  Hs_i = h [[1,-1],[-1,1]]
 //   geomean:        Hs_i = M (diag(w_act) - w_act w_act'/W_act)
+//   n-coin StableSwap: Hs_i = C - (C1)(C1)'/(1'C1), C = diag(h^2) - h h'/(1 + k)   (cfmm_small::stableswap_n)
 // ---------------------------------------------------------------------------------------------
 template <typename Scatter>
 __global__ void __launch_bounds__(kThreads)
@@ -530,6 +572,86 @@ k_dense_geomean(long long m, long long ld, int k, int n, const int* __restrict__
     }
 }
 
+// n-coin StableSwap: Hs_TT = C - (C1)(C1)' / (1'C1), C = diag(h^2) - h h' / (1 + k), from the per-slot h (hcoef
+// [arity][ld], 0 off the traded set T, k = |T|); O(arity) per pool (cfmm_small::stablen_hvp).
+template <typename Scatter>
+__global__ void __launch_bounds__(kThreads)
+k_hvp_stable_n(long long m, long long ld, int k, int n_tokens, const int* __restrict__ idx,
+               const double* __restrict__ hcoef, const uint32_t* __restrict__ hmask, const double* __restrict__ vt,
+               double* y) {
+    extern __shared__ double smem[];
+    Scatter sc{y};
+    sc.init(smem, n_tokens);
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        if (!hmask[i]) continue;
+        double h[cfmm_small::KMAX], z[cfmm_small::KMAX], out[cfmm_small::KMAX];
+        int id[cfmm_small::KMAX];
+#pragma unroll
+        for (int j = 0; j < cfmm_small::KMAX; ++j) {
+            if (j < k) {
+                id[j] = idx[(long long)j * ld + i];
+                h[j] = hcoef[(long long)j * ld + i];
+                z[j] = __ldg(vt + id[j]);
+            }
+        }
+        cfmm_small::stablen_hvp<cfmm_small::KMAX>(k, h, z, out);
+#pragma unroll
+        for (int j = 0; j < cfmm_small::KMAX; ++j)
+            if (j < k && h[j] != 0.0) sc.add(id[j], out[j]);
+    }
+    sc.flush(smem, n_tokens);
+}
+
+// the (C1)_j and 1'C1 of pool i's block (cfmm_small::stablen_c1), h loaded from hcoef [arity][ld]
+__device__ __forceinline__ double stable_n_c1(long long i, long long ld, int k, const double* __restrict__ hcoef,
+                                              double* h, double* c1, double& inv) {
+#pragma unroll
+    for (int j = 0; j < cfmm_small::KMAX; ++j)
+        if (j < k) h[j] = hcoef[(long long)j * ld + i];
+    return cfmm_small::stablen_c1<cfmm_small::KMAX>(k, h, c1, inv);
+}
+
+// diagonal: C_jj - (C1)_j^2 / (1'C1), C_jj = h_j^2 k / (1 + k)
+__global__ void __launch_bounds__(kThreads)
+k_diag_stable_n(long long m, long long ld, int k, const int* __restrict__ idx, const double* __restrict__ hcoef,
+                const uint32_t* __restrict__ hmask, double* diag) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        if (!hmask[i]) continue;
+        double h[cfmm_small::KMAX], c1[cfmm_small::KMAX], inv;
+        const double s1 = stable_n_c1(i, ld, k, hcoef, h, c1, inv);
+        if (!(s1 > 0.0)) continue;
+#pragma unroll
+        for (int j = 0; j < cfmm_small::KMAX; ++j)
+            if (j < k && h[j] != 0.0)
+                atomicAdd(diag + idx[(long long)j * ld + i], h[j] * h[j] * (1.0 - inv) - c1[j] * c1[j] / s1);
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_dense_stable_n(long long m, long long ld, int k, int n, const int* __restrict__ idx, const double* __restrict__ hcoef,
+                 const uint32_t* __restrict__ hmask, double* H) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        if (!hmask[i]) continue;
+        double h[cfmm_small::KMAX], c1[cfmm_small::KMAX], inv;
+        const double s1 = stable_n_c1(i, ld, k, hcoef, h, c1, inv);
+        if (!(s1 > 0.0)) continue;
+#pragma unroll
+        for (int x = 0; x < cfmm_small::KMAX; ++x) {
+            if (x >= k || h[x] == 0.0) continue;
+            const long long tx = idx[(long long)x * ld + i];
+#pragma unroll
+            for (int y = 0; y < cfmm_small::KMAX; ++y) {
+                if (y >= k || h[y] == 0.0) continue;
+                const long long ty = idx[(long long)y * ld + i];
+                atomicAdd(H + tx * n + ty, (x == y ? h[x] * h[x] : 0.0) - h[x] * h[y] * inv - c1[x] * c1[y] / s1);
+            }
+        }
+    }
+}
+
 __global__ void __launch_bounds__(kThreads)
 k_sum_update(long long m, long long ld, const double* __restrict__ R, const double* __restrict__ lambda,
              double* thbar, double* move) {
@@ -635,6 +757,40 @@ int launch_stable(const cfmm_bucket* b, int n_tokens, const double* nu, double* 
     return check_launch();
 }
 
+// n-coin StableSwap buckets: the LDG path only, as for two coins
+template <int K, bool TRADES, bool HESS>
+int launch_stable_n(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                    const cfmm_eval_out* out, cudaStream_t st) {
+    const long long m = b->n_pools;
+    double* delta = out ? out->delta : nullptr;
+    double* lambda = out ? out->lambda : nullptr;
+    double* hcoef = out ? out->hcoef : nullptr;
+    uint32_t* hmask = out ? out->hmask : nullptr;
+    if (use_shared(n_tokens, m * K / 2)) {
+        const size_t sm = (size_t)n_tokens * sizeof(double);
+        auto kern = k_eval_stable_n<K, SharedScatter, TRADES, HESS>;
+        allow_smem(kern, sm);
+        kern<<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights,
+                                                    b->logrw, nu, psi, arb, delta, lambda, hcoef, hmask);
+    } else {
+        k_eval_stable_n<K, GlobalScatter, TRADES, HESS><<<grid_for(m, 4), kThreads, 0, st>>>(
+            m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights, b->logrw, nu, psi, arb, delta, lambda,
+            hcoef, hmask);
+    }
+    return check_launch();
+}
+
+template <int K>
+int dispatch_stable_n(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                      const cfmm_eval_out* out, cudaStream_t st) {
+    const bool trades = out && out->delta && out->lambda;
+    const bool hess = out && out->hcoef && out->hmask;
+    if (trades && hess) return launch_stable_n<K, true, true>(b, n_tokens, nu, psi, arb, out, st);
+    if (trades) return launch_stable_n<K, true, false>(b, n_tokens, nu, psi, arb, out, st);
+    if (hess) return launch_stable_n<K, false, true>(b, n_tokens, nu, psi, arb, out, st);
+    return launch_stable_n<K, false, false>(b, n_tokens, nu, psi, arb, out, st);
+}
+
 template <int KIND, bool TRADES, bool HESS>
 int launch_kind(const cfmm_bucket* b, int n_tokens, const double* nu, double eps, double* psi, double* arb,
                 const cfmm_eval_out* out, cudaStream_t st) {
@@ -710,6 +866,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 2) return CFMM_E_KIND;
             if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // rates; (A, D)
             break;
+        case CFMM_KIND_STABLESWAP_N:
+            if (b->arity < 2 || b->arity > 8) return CFMM_E_KIND;
+            if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // rates; (A, D)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -739,6 +899,16 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_BOUNDED_PRODUCT>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP:
             return dispatch_pair<CFMM_KIND_STABLESWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_STABLESWAP_N:
+            switch (b->arity) {
+                case 2: return dispatch_stable_n<2>(b, n_tokens, nu, psi, arb, out, st);
+                case 3: return dispatch_stable_n<3>(b, n_tokens, nu, psi, arb, out, st);
+                case 4: return dispatch_stable_n<4>(b, n_tokens, nu, psi, arb, out, st);
+                case 5: return dispatch_stable_n<5>(b, n_tokens, nu, psi, arb, out, st);
+                case 6: return dispatch_stable_n<6>(b, n_tokens, nu, psi, arb, out, st);
+                case 7: return dispatch_stable_n<7>(b, n_tokens, nu, psi, arb, out, st);
+                default: return dispatch_stable_n<8>(b, n_tokens, nu, psi, arb, out, st);
+            }
         default:
             break;
     }
@@ -765,7 +935,17 @@ int cfmm_hvp(const cfmm_bucket* b, int32_t n_tokens, const double* hcoef, const 
     const long long m = b->n_pools;
     const bool sh = use_shared(n_tokens, m * b->arity / 2);
     const size_t sm = sh ? (size_t)n_tokens * sizeof(double) : 0;
-    if (b->kind == CFMM_KIND_GEOMEAN) {
+    if (b->kind == CFMM_KIND_STABLESWAP_N) {
+        if (!hmask) return CFMM_E_NULL;
+        if (sh) {
+            allow_smem(k_hvp_stable_n<SharedScatter>, sm);
+            k_hvp_stable_n<SharedScatter><<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, b->arity, n_tokens,
+                                                                                b->tok_idx, hcoef, hmask, vt, y);
+        } else {
+            k_hvp_stable_n<GlobalScatter><<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, n_tokens,
+                                                                               b->tok_idx, hcoef, hmask, vt, y);
+        }
+    } else if (b->kind == CFMM_KIND_GEOMEAN) {
         if (!hmask) return CFMM_E_NULL;
         if (sh) {
             allow_smem(k_hvp_geomean<SharedScatter>, sm);
@@ -794,7 +974,10 @@ int cfmm_hess_diag(const cfmm_bucket* b, int32_t n_tokens, const double* hcoef, 
     if (b->n_pools == 0) return CFMM_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long m = b->n_pools;
-    if (b->kind == CFMM_KIND_GEOMEAN) {
+    if (b->kind == CFMM_KIND_STABLESWAP_N) {
+        if (!hmask) return CFMM_E_NULL;
+        k_diag_stable_n<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, b->tok_idx, hcoef, hmask, diag);
+    } else if (b->kind == CFMM_KIND_GEOMEAN) {
         if (!hmask) return CFMM_E_NULL;
         k_diag_geomean<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, b->tok_idx, b->weights, hcoef, hmask, diag);
     } else {
@@ -811,7 +994,11 @@ int cfmm_hess_dense(const cfmm_bucket* b, int32_t n_tokens, const double* hcoef,
     if (b->n_pools == 0) return CFMM_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long m = b->n_pools;
-    if (b->kind == CFMM_KIND_GEOMEAN) {
+    if (b->kind == CFMM_KIND_STABLESWAP_N) {
+        if (!hmask) return CFMM_E_NULL;
+        k_dense_stable_n<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, n_tokens, b->tok_idx, hcoef, hmask,
+                                                               H);
+    } else if (b->kind == CFMM_KIND_GEOMEAN) {
         if (!hmask) return CFMM_E_NULL;
         k_dense_geomean<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, n_tokens, b->tok_idx, b->weights, hcoef,
                                                               hmask, H);

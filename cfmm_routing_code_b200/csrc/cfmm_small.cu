@@ -18,7 +18,8 @@ constexpr int kSmallThreads = 32;     // one warp per CTA: a sweep of 50 problem
 // loop of every evaluation split over the lanes (latency: a handful of problems, or problems with hundreds of pools);
 // each lane keeps its own copy of the state at work[(p * LANES + lane)], so `stride` counts lanes, not problems.
 // STABLE: also evaluate StableSwap pools (k_batch_solve_stable); without it such a pool makes its problem status 3.
-template <int LANES, bool STABLE>
+// STABLE_N: StableSwap pools of 2..8 coins (k_batch_solve_stable_n).
+template <int LANES, bool STABLE, bool STABLE_N = false>
 __device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, const cfmm_batch& B, const cfmm_small::Params& prm,
                                                  int n, long long n_pools, double* work, long long stride) {
     const long long gt = (long long)blockIdx.x * kSmallThreads + threadIdx.x;
@@ -43,8 +44,8 @@ __device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, con
     Q.flags = B.flags + p * n;
     Q.delta = B.delta ? B.delta + p * B.trade_stride : nullptr;
     Q.lam = B.lambda ? B.lambda + p * B.trade_stride : nullptr;
-    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE>(P, Q, prm, B.nu + p * n, B.psi + p * n,
-                                                                     work + (LANES == 1 ? p : p * LANES + lane), stride, lane);
+    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE, STABLE_N>(P, Q, prm, B.nu + p * n, B.psi + p * n,
+                                                                               work + (LANES == 1 ? p : p * LANES + lane), stride, lane);
     if (lane == 0) {
         st[0] = r.value; st[1] = r.dual; st[2] = r.gap; st[3] = r.infeas; st[4] = r.err;
         st[5] = (double)r.iters; st[6] = (double)r.evals; st[7] = (double)r.status;
@@ -65,6 +66,15 @@ __global__ void __launch_bounds__(kSmallThreads)
 k_batch_solve_stable(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm, int n, long long n_pools, double* work,
                      long long stride) {
     batch_solve_body<LANES, true>(P, B, prm, n, n_pools, work, stride);
+}
+
+// and for pool sets with StableSwap pools of more than two coins: a third instance, so that the n-coin evaluation
+// (cfmm_small::stableswap_n) leaves the other two instances' registers as they are
+template <int LANES>
+__global__ void __launch_bounds__(kSmallThreads)
+k_batch_solve_stable_n(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm, int n, long long n_pools, double* work,
+                       long long stride) {
+    batch_solve_body<LANES, true, true>(P, B, prm, n, n_pools, work, stride);
 }
 
 int g_batch_lanes = 1;       // cfmm_set_batch_lanes: 1 | 32
@@ -88,7 +98,7 @@ extern "C" int cfmm_set_batch_lanes(int32_t lanes) {
 
 namespace {
 int batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm, void* work,
-                void* stream, bool stable) {
+                void* stream, int stable) {
     if (!pools || !batch || !prm) return CFMM_E_NULL;
     if (batch->n_problems == 0) return CFMM_OK;
     if (!pools->pool_ptr || !pools->tok_idx || !pools->reserves || !pools->weights || !pools->logrw || !pools->gamma ||
@@ -103,7 +113,14 @@ int batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm
     const long long stride = padded(batch->n_problems) * g_batch_lanes;      // state slots = CUDA threads
     const unsigned grid = (unsigned)(stride / kSmallThreads);
     cudaStream_t st = (cudaStream_t)stream;
-    if (stable) {
+    if (stable == 2) {
+        if (g_batch_lanes == 32)
+            k_batch_solve_stable_n<32><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools,
+                                                                       (double*)work, stride);
+        else
+            k_batch_solve_stable_n<1><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools,
+                                                                      (double*)work, stride);
+    } else if (stable == 1) {
         if (g_batch_lanes == 32)
             k_batch_solve_stable<32><<<grid, kSmallThreads, 0, st>>>(P, *batch, q, pools->n_tokens, pools->n_pools,
                                                                      (double*)work, stride);
@@ -123,10 +140,15 @@ int batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm
 
 extern "C" int cfmm_batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
                                 void* work, void* stream) {
-    return batch_solve(pools, batch, prm, work, stream, false);
+    return batch_solve(pools, batch, prm, work, stream, 0);
 }
 
 extern "C" int cfmm_batch_solve_stableswap(const cfmm_csr_pools* pools, const cfmm_batch* batch,
                                            const cfmm_batch_params* prm, void* work, void* stream) {
-    return batch_solve(pools, batch, prm, work, stream, true);
+    return batch_solve(pools, batch, prm, work, stream, 1);
+}
+
+extern "C" int cfmm_batch_solve_stableswap_n(const cfmm_csr_pools* pools, const cfmm_batch* batch,
+                                             const cfmm_batch_params* prm, void* work, void* stream) {
+    return batch_solve(pools, batch, prm, work, stream, 2);
 }

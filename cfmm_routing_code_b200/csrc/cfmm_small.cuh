@@ -18,8 +18,10 @@
 
 #ifdef __CUDACC__
 #define CFMM_HD __host__ __device__
+#define CFMM_UNROLL _Pragma("unroll")
 #else
 #define CFMM_HD
+#define CFMM_UNROLL
 #endif
 
 namespace cfmm_small {
@@ -37,7 +39,8 @@ struct Pools {                       // CSR problem data (device pointers in the
                                      //         rates (kind 4)
     const double* logrw;             // [nnz]   log(R/w) | kind 4: A at the pool's first slot, its invariant D at the second
     const double* gamma;             // [m]     fees                           arbitrage.py:22-28
-    const uint8_t* kind;             // [m]     1 = constant sum; 3 = bounded-liquidity product; 4 = two-coin StableSwap;
+    const uint8_t* kind;             // [m]     1 = constant sum; 3 = bounded-liquidity product; 4 = StableSwap (2 coins;
+                                     //         2..KMAX in the STABLE_N instance);
                                      //         0 or 2 = weighted geometric mean
                                      //         (constant product = equal weights)
 };
@@ -183,11 +186,235 @@ CFMM_HD inline void stableswap_pair(double R0, double R1, double r0, double r1, 
     D[0] = d0; D[1] = d1; L[0] = l0; L[1] = l1;
 }
 
+// n-coin StableSwap (Curve) pool, n = k = 2..KM coins.  Scaled balances y_j = r_j x_j, whitepaper amplification A,
+// a = A n^n, and D = D(R) the invariant of the current reserves (precomputed).  In units of D (u_j = y_j / D) the pool
+// keeps G(u) = a sum(u) + 1 - a - Q(u) >= 0, Q(u) = 1 / (n^n prod u); G is strictly concave on u > 0 and
+// dG/du_j = a + Q / u_j.  With pi_j = nu_j / r_j a coordinate that grows pays p_j = pi_j / gamma per unit of u, one that
+// shrinks earns p_j = pi_j, and the pool solves max -sum_j p_j(u_j - u0_j) s.t. G(u) >= 0.
+//   No trade: rho_j = pi_j / dG/du_j(u0); the pool is idle iff gamma max rho <= min rho (in logs: c_j = log(pi_j /
+//   pi_min) - log1p(Q0 / (a u0_j)), idle iff log gamma + max c <= min c).  Flows and h are then exactly 0.
+//   Otherwise, for the multiplier mu of G and the value Q, the Lagrangian's stationary point is
+//       u_j(mu, Q) = clamp(u0_j, Q / (pi_j / (gamma mu) - a), Q / (pi_j / mu - a))     (a denominator <= 0: +inf).
+//   Near the peg with large a, pi_j / mu - a must not be formed as a difference: with dB_j = log(pi_j / pi_min) >= 0
+//   and the unknown tau = log(pi_min / (gamma a mu)) > 0, the denominators are a expm1(dB_j + tau) and
+//   a expm1(dB_j + log gamma + tau), without cancellation.  With l = log(Q / a), l0 = log(Q0 / a):
+//       log u_j = log u0_j + z_j,   z_j = max(l - bA_j, 0) + min(l - bB_j, 0),
+//       bA_j = log(u0_j expm1(dB_j + tau)),   bB_j = log(u0_j expm1(dB_j + log gamma + tau))  (-inf if that expm1 <= 0),
+//   and Q = Q(u) reads F(l) = (l - l0) + sum_j z_j(l) = 0: piecewise linear with slope >= 1, so its root is exact from
+//   the 2n breakpoints (as k_eval_geomean's).  h(tau) = sum_j u0_j expm1(z_j) - q0 expm1(l - l0) = G / a at that point
+//   (formed from the changes, not from a sum(u) + 1 - a - Q) falls from +inf (tau -> 0) to -inf (tau -> inf); its root
+//   is found by bracketing and a bisection-safeguarded Newton iteration in log tau (the stableswap_dir scheme), with
+//   dh/dtau = sum_T u_j (l' - kap_j) - q l', kap_j = 1 + 1 / expm1(.)_j, l' = sum_T kap_j / (1 + k) over the traded set T.
+//   Then x_j = R_j exp(z_j): D_j = R_j expm1(z_j) / gamma, L_j = -R_j expm1(z_j).
+// Hessian.  Differentiating the KKT system p_j = mu dG/du_j (j in T), G = 0: with w = 1/u, -d2G_TT = Q (diag(w^2) + w w'),
+// so by Sherman-Morrison its inverse is (diag(u^2) - u u' / (1 + k)) / Q, and eliminating dmu gives the scaled Hessian
+// Hs_ij = nu_i nu_j dpsi_i/dnu_j on T x T:
+//       v_j = p_j u_j,  c = D / (mu Q),  h_j = sqrt(c) v_j,  C = diag(h^2) - h h' / (1 + k),
+//       Hs_TT = C - (C1)(C1)' / (1'C1),   zero outside T.
+// It is PSD, Hs 1 = 0, and Hs z costs O(k): Cz = h^2 z - h (h.z) / (1 + k), C1 = h^2 - h sum(h) / (1 + k),
+// 1'C1 = sum(h^2) - sum(h)^2 / (1 + k).  Here mu Q = pi_min e^-tau q / gamma (q = Q / a), so c = D gamma e^tau / (pi_min q).
+// Arrays of KM entries with the first k used, every loop unrolled over KM: the kernel keeps them in registers.
+// Writes D, L and h (0 on untraded slots) and returns the traded slots as a bit mask.  Fixed iteration caps and a
+// deterministic exit; shared by the per-thread solver and k_eval_stable_n (cfmm_kernels.cu).
+
+// h(tau) / a at tau = exp(sg), and dh/dsg; z [KM] and l out.  sc: the rounding scale of h (stopping rule)
+template <int KM>
+CFMM_HD inline double stablen_h(int k, double sg, const double* dB, double lg, const double* u0, const double* lu0,
+                                double l0, double q0, double* z, double& l, double& dh, double& sc) {
+    const double tau = exp(sg);
+    double eA[KM], eB[KM], bA[KM], bB[KM];
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j) {
+        if (j < k) {
+            eA[j] = expm1(dB[j] + tau);
+            eB[j] = expm1(dB[j] + lg + tau);
+            bA[j] = lu0[j] + log(eA[j]);
+            bB[j] = eB[j] > 0.0 ? lu0[j] + log(eB[j]) : -INFINITY;
+        }
+    }
+    // the largest breakpoint with F <= 0 (sL, F there), and the smallest one (sM, F there)
+    double sL = -INFINITY, FL = 0.0, sM = INFINITY, FM = 0.0;
+CFMM_UNROLL
+    for (int p = 0; p < 2 * KM; ++p) {
+        if ((p < KM ? p : p - KM) < k) {
+            const double T = p < KM ? bA[p] : bB[p - KM];
+            if (fabs(T) < INFINITY) {
+                double F = T - l0;
+CFMM_UNROLL
+                for (int j = 0; j < KM; ++j)
+                    if (j < k) F += fmax(T - bA[j], 0.0) + fmin(T - bB[j], 0.0);
+                if (F <= 0.0 && T > sL) { sL = T; FL = F; }
+                if (T < sM) { sM = T; FM = F; }
+            }
+        }
+    }
+    double slope = 1.0;
+    if (sL > -INFINITY) {
+CFMM_UNROLL
+        for (int j = 0; j < KM; ++j)
+            if (j < k) slope += (sL >= bA[j] ? 1.0 : 0.0) + (sL < bB[j] ? 1.0 : 0.0);
+        l = sL - FL / slope;
+    } else {                                    // left of every breakpoint only the finite bB bind
+CFMM_UNROLL
+        for (int j = 0; j < KM; ++j)
+            if (j < k) slope += bB[j] > -INFINITY ? 1.0 : 0.0;
+        l = sM - FM / slope;
+    }
+    const double q = q0 * exp(l - l0);
+    double h = -q0 * expm1(l - l0), skap = 0.0, su = 0.0, suk = 0.0;
+    int kt = 0;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j) {
+        if (j < k) {
+            z[j] = fmax(l - bA[j], 0.0) + fmin(l - bB[j], 0.0);
+            h += u0[j] * expm1(z[j]);
+            const double u = u0[j] * exp(z[j]);
+            su += u;
+            if (z[j] != 0.0) {
+                const double kap = 1.0 + 1.0 / (z[j] > 0.0 ? eA[j] : eB[j]);
+                ++kt; skap += kap; suk += u * kap;
+            }
+        }
+    }
+    double sut = 0.0;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j)
+        if (j < k && z[j] != 0.0) sut += u0[j] * exp(z[j]);
+    const double lt = skap / (1.0 + kt);
+    dh = tau * (sut * lt - suk - q * lt);
+    sc = (su + q) * (1.0 + fabs(l));
+    return h;
+}
+
+template <int KM>
+CFMM_HD inline uint32_t stableswap_n(int k, const double* R, const double* r, double A, double Dv, double gam,
+                                     const double* nu, double* D, double* L, double* hs) {
+    double u0[KM], lu0[KM], pi[KM], dB[KM], z[KM];
+    double nn = 1.0, slu = 0.0, pmin = INFINITY;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j) {
+        if (j < k) {
+            nn *= (double)k;
+            D[j] = L[j] = hs[j] = 0.0;
+            u0[j] = r[j] * R[j] / Dv;
+            lu0[j] = log(u0[j]);
+            slu += lu0[j];
+            pi[j] = nu[j] / r[j];
+            pmin = fmin(pmin, pi[j]);
+        }
+    }
+    const double a = A * nn;
+    const double l0 = -((double)k * log((double)k) + slu) - log(a), q0 = exp(l0), lg = log(gam);
+    double cmax = -INFINITY, cmin = INFINITY;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j) {
+        if (j < k) {
+            dB[j] = log(pi[j] / pmin);
+            const double c = dB[j] - log1p(q0 / u0[j]);
+            cmax = fmax(cmax, c);
+            cmin = fmin(cmin, c);
+        }
+    }
+    if (!(lg + cmax > cmin)) return 0u;                                 // the no-trade band: exactly nothing
+    constexpr double SMIN = -700.0, SMAX = 6.39;                        // log tau: tau in (1e-304, 600), exp finite
+    double l = 0.0, dh = 0.0, sc = 0.0;
+    // start where the last grower stops growing at Q = Q0, then bracket: h(lo) > 0 >= h(hi)
+    const double sg = fmin(fmax(log(-cmin), SMIN), SMAX);
+    double lo = sg, hi = sg;
+    if (stablen_h<KM>(k, sg, dB, lg, u0, lu0, l0, q0, z, l, dh, sc) > 0.0) {
+        for (double step = 1.0; step <= 512.0 && lo < SMAX; step *= 2.0) {
+            hi = fmin(lo + step, SMAX);
+            if (!(stablen_h<KM>(k, hi, dB, lg, u0, lu0, l0, q0, z, l, dh, sc) > 0.0)) break;
+            lo = hi;
+        }
+    } else {
+        for (double step = 1.0; step <= 512.0 && hi > SMIN; step *= 2.0) {
+            lo = fmax(hi - step, SMIN);
+            if (stablen_h<KM>(k, lo, dB, lg, u0, lu0, l0, q0, z, l, dh, sc) > 0.0) break;
+            hi = lo;
+        }
+    }
+    // safeguarded Newton inside [lo, hi] (h falls in log tau), as stableswap_dir
+    double t = 0.5 * (lo + hi), dx_old = hi - lo, dx = dx_old;
+    for (int it = 0; it < 100; ++it) {
+        const double f = stablen_h<KM>(k, t, dB, lg, u0, lu0, l0, q0, z, l, dh, sc);
+        if (f > 0.0) lo = t; else hi = t;
+        if (f == 0.0 || !(hi - lo > 4e-16 * (1.0 + fabs(t)))) break;
+        const double tn = t - f / dh;
+        // h is at the level of its own rounding (the z_j carry absolute errors of a few u |l|): stop there
+        if (fabs(f) <= 4.5e-16 * sc) {
+            if (tn > lo && tn < hi) t = tn;
+            break;
+        }
+        if (!(tn > lo && tn < hi) || fabs(2.0 * f) > fabs(dx_old * dh)) {
+            dx_old = dx; dx = 0.5 * (hi - lo); t = lo + dx;
+        } else {
+            dx_old = dx; dx = tn - t; t = tn;
+        }
+        if (fabs(dx) <= 1e-15 * (1.0 + fabs(t))) break;
+    }
+    stablen_h<KM>(k, t, dB, lg, u0, lu0, l0, q0, z, l, dh, sc);
+    const double q = q0 * exp(l - l0);
+    const double sc_h = sqrt(Dv * gam * exp(exp(t)) / (pmin * q));
+    uint32_t mask = 0u;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j) {
+        if (j < k && z[j] != 0.0) {
+            const double e = expm1(z[j]);
+            if (z[j] > 0.0) D[j] = R[j] * e / gam; else L[j] = -R[j] * e;
+            hs[j] = sc_h * (z[j] > 0.0 ? pi[j] / gam : pi[j]) * u0[j] * exp(z[j]);
+            mask |= 1u << j;
+        }
+    }
+    return mask;
+}
+
+// The pieces of one n-coin StableSwap pool's block Hs = C - (C1)(C1)' / (1'C1), C = diag(h^2) - h h' / (1 + k), from its
+// per-slot h (0 off the traded set T, k = |T|): c1 [KM] = C1 (0 off T), inv = 1 / (1 + k); returns 1'C1 (<= 0: fewer
+// than two traded slots, the block is 0).  Shared by the per-thread solver's dense assembly, stablen_hvp and the diagonal
+// and dense kernels of cfmm_kernels.cu.
+template <int KM>
+CFMM_HD inline double stablen_c1(int k, const double* h, double* c1, double& inv) {
+    double sh = 0.0, sh2 = 0.0;
+    int kt = 0;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j)
+        if (j < k && h[j] != 0.0) { ++kt; sh += h[j]; sh2 += h[j] * h[j]; }
+    inv = 1.0 / (1.0 + kt);
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j)
+        if (j < k) c1[j] = h[j] * h[j] - h[j] * sh * inv;
+    return sh2 - sh * sh * inv;
+}
+
+// Hs z for one n-coin StableSwap pool from its per-slot h: (Hs z)_j, j < k, into y.  O(k): Cz = h^2 z - h (h.z) / (1 + k)
+// and (C1)'z = 1'Cz.
+template <int KM>
+CFMM_HD inline void stablen_hvp(int k, const double* h, const double* zin, double* y) {
+    double c1[KM], inv;
+    const double s1 = stablen_c1<KM>(k, h, c1, inv);
+    double shz = 0.0, c1z = 0.0;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j)
+        if (j < k) shz += h[j] * zin[j];
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j) {
+        if (j < k) {
+            y[j] = h[j] * h[j] * zin[j] - h[j] * shz * inv;                // (Cz)_j
+            c1z += y[j];
+        }
+    }
+    const double f = s1 > 0.0 ? c1z / s1 : 0.0;
+CFMM_UNROLL
+    for (int j = 0; j < KM; ++j)
+        if (j < k) y[j] = s1 > 0.0 ? y[j] - c1[j] * f : 0.0;
+}
+
 #ifdef __CUDA_ARCH__
 // sum over the LANES consecutive lanes that share a problem; x + y == y + x exactly, so every lane ends with the same bits
 template <int LANES>
 __device__ __forceinline__ double lanes_sum(double v) {
-#pragma unroll
+CFMM_UNROLL
     for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
@@ -202,7 +429,10 @@ __device__ __forceinline__ double lanes_sum(double v) {
 // bit-identical totals in every lane -- so the lanes never diverge and need no other communication.
 // STABLE: the instance that also evaluates StableSwap pools (kind 4).  The plain instance keeps the register budget it
 // had before that kind existed and rejects such pools (solve_one: status 3); cfmm_batch_solve_stableswap runs the other.
-template <int LANES, bool STABLE = false>
+// STABLE_N (with STABLE): kind-4 pools of 2..KMAX coins, those of more than two through stableswap_n, whose k x k block
+// of Hs is added to the dense system; cfmm_batch_solve_stableswap_n runs this third instance.  Without it a kind-4 pool
+// of more than two coins makes its problem status 3.
+template <int LANES, bool STABLE = false, bool STABLE_N = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane) {
     const int n = Q.n;
@@ -218,7 +448,27 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
         const int k = (int)(P.pool_ptr[i + 1] - off);
         const double gam = P.gamma[i];
         double D[KMAX], L[KMAX];
-        if (P.kind[i] == 3 || (STABLE && P.kind[i] == 4)) {
+        if (STABLE_N && P.kind[i] == 4 && k > 2) {                       // rates in w, (A, D) in logrw's first two slots
+            double Rl[KMAX], rl[KMAX], nl[KMAX], hl[KMAX];
+            for (int j = 0; j < KMAX; ++j) {
+                if (j < k) { Rl[j] = P.R[off + j]; rl[j] = P.w[off + j]; nl[j] = nu[P.tok[off + j]]; }
+            }
+            stableswap_n<KMAX>(k, Rl, rl, P.logrw[off], P.logrw[off + 1], gam, nl, D, L, hl);
+            if (Hs) {                                                      // Hs_TT = C - (C1)(C1)' / (1'C1)
+                double c1[KMAX], inv;
+                const double s1 = stablen_c1<KMAX>(k, hl, c1, inv);
+                if (s1 > 0.0) {
+                    for (int x = 0; x < k; ++x) {
+                        if (hl[x] == 0.0) continue;
+                        const int tx = P.tok[off + x];
+                        for (int y = 0; y < k; ++y) {
+                            if (hl[y] == 0.0) continue;
+                            (*Hs)[tx * n + P.tok[off + y]] += (x == y ? hl[x] * hl[x] : 0.0) - hl[x] * hl[y] * inv - c1[x] * c1[y] / s1;
+                        }
+                    }
+                }
+            }
+        } else if (P.kind[i] == 3 || (STABLE && P.kind[i] == 4)) {
             double hc = 0.0;
             if (!STABLE || P.kind[i] == 3)
                 bounded_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], gam, nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
@@ -416,7 +666,7 @@ CFMM_HD inline int newton_direction(int n, uint64_t free_mask, const Vec& Hs, co
 CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL * n * n + (int64_t)n * (n + 1) + 2 * nnz; }
 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
-template <int LANES = 1, bool STABLE = false>
+template <int LANES = 1, bool STABLE = false, bool STABLE_N = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0) {
     const int n = Q.n;
@@ -437,7 +687,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1;
         bad = P.kind[i] > (STABLE ? 4 : 3) || k < 2 || k > KMAX ||
-              ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && P.kind[i] == 4)) && k != 2);
+              ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4)) && k != 2);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
     if (bad) {
@@ -464,7 +714,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -510,7 +760,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -535,8 +785,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
+        evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -561,8 +811,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
+    evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

@@ -186,6 +186,51 @@ def synth_stable_market(m, n_tokens, seed, frac_stable=0.3, frac_weighted=0.1, n
     )
 
 
+def synth_stable_n_market(m, n_tokens, seed, frac_stable=0.3, n_stable=8, mispricing=0.02, arities=(2, 3, 4)):
+    """A market with StableSwap clusters of several coin counts: tokens 0..n_stable-1 trade near 1 (within +-0.2 %),
+    the last two of them rate-bearing (worth 1.02 / 1.05 of the others).  StableSwap pools of each arity in `arities`
+    (in equal shares, tokens drawn from the cluster without repetition; whitepaper A with A n^n in 100 .. 2e4, the
+    coefficients of Curve's usual A() = 50 .. 5000 at n = 2..4; rates = the tokens' values) sit beside constant-product
+    pools over all tokens, the cluster included.  Balances are value-imbalanced by up to ~2x and mispriced by
+    `mispricing`.  Returns CSR arrays (HostPools(**out) minus `prices`) plus the prices."""
+    rng = np.random.default_rng(seed)
+    n_stable = min(n_stable, n_tokens)
+    arities = [k for k in arities if k <= n_stable]
+    p = np.exp(rng.standard_normal(n_tokens))
+    rate = np.ones(n_tokens)
+    rate[max(0, n_stable - 2):n_stable] = [1.02, 1.05][-min(2, n_stable):]
+    p[:n_stable] = rate[:n_stable] * np.exp(0.002 * rng.uniform(-1, 1, n_stable))
+    n_ss = int(round(frac_stable * m)) if arities else 0
+    n_cp = m - n_ss
+    a = rng.integers(0, n_tokens, n_cp); b = (a + rng.integers(1, n_tokens, n_cp)) % n_tokens
+    liq = np.exp(8.0 + 1.5 * rng.standard_normal(n_cp))
+    out_idx = [np.stack([a, b], 1)]
+    out_R = [np.stack([liq / p[a], liq / p[b]], 1) * np.exp(mispricing * rng.standard_normal((n_cp, 2)))]
+    out_w = [np.full((n_cp, 2), 0.5)]; out_g = [_FEES[rng.integers(0, 3, n_cp)]]; out_k = [np.zeros(n_cp, np.uint8)]
+    out_ar = [np.full(n_cp, 2)]; out_amp = [np.zeros(n_cp)]
+    for x, k in enumerate(arities):
+        mk = n_ss // len(arities) + (1 if x < n_ss % len(arities) else 0)
+        if mk == 0:
+            continue
+        toks = np.argsort(rng.random((mk, n_stable)), 1)[:, :k]
+        V = np.exp(9.0 + 1.5 * rng.standard_normal(mk))
+        imb = np.exp(0.35 * rng.standard_normal((mk, k)))
+        out_idx.append(toks)
+        out_R.append(V[:, None] * imb / p[toks] * np.exp(mispricing * rng.standard_normal((mk, k))))
+        out_w.append(rate[toks]); out_g.append(np.array([0.9996, 0.9999, 0.99995])[rng.integers(0, 3, mk)])
+        out_k.append(np.full(mk, 4, np.uint8)); out_ar.append(np.full(mk, k))
+        out_amp.append(np.array([100.0, 1000.0, 2e4])[rng.integers(0, 3, mk)] / float(k ** k))
+    arity = np.concatenate(out_ar)
+    return dict(
+        n_tokens=n_tokens, prices=p,
+        pool_ptr=np.concatenate([[0], np.cumsum(arity)]).astype(np.int64),
+        tok_idx=np.concatenate([x.ravel() for x in out_idx]).astype(np.int32),
+        reserves=np.concatenate([x.ravel() for x in out_R]),
+        weights=np.concatenate([x.ravel() for x in out_w]),
+        gamma=np.concatenate(out_g), kind=np.concatenate(out_k), amp=np.concatenate(out_amp),
+    )
+
+
 def synth_basket(n_tokens, prices, seed, n_assets=16, scale=1e-3, liq_mean=np.exp(8.0)):
     """cfg 4 basket: a_j = exp(N(0,1)) * Lbar / p_j * 1e-3 on 16 random tokens, target token 0."""
     rng = np.random.default_rng(seed)

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+import functools
 from collections.abc import Mapping
 from typing import Dict, List, Optional, Sequence
 
@@ -19,13 +20,15 @@ from . import _lib
 KIND_GEOMEAN_HOST = 0   # host CSR convention: 0 = (weighted) geometric mean, 1 = constant sum
 KIND_SUM_HOST = 1
 KIND_BOUNDED_HOST = 3   # constant product on virtual reserves (reserves + offsets), real reserves >= 0; offsets ride in `weights`
-KIND_STABLESWAP_HOST = 4  # two-coin StableSwap (Curve); rates ride in `weights`, the amplification in HostPools.amp
-AMP_MAX = 1e7           # largest StableSwap amplification A accepted
+KIND_STABLESWAP_HOST = 4  # StableSwap (Curve), 2..8 coins; rates ride in `weights`, the amplification in HostPools.amp
+ANN_MAX = 4e7           # largest StableSwap coefficient A n^n accepted, any coin count (A <= 1e7 for two coins)
+STABLE_ARITY_MAX = 8    # most coins of a StableSwap pool
 
 
 def stableswap_invariant(reserves, rates, amp) -> np.ndarray:
     """Invariant D of two-coin StableSwap pools: the root of 4A (y0 + y1) + D = 4A D + D^3 / (4 y0 y1) with the scaled
-    balances y = rates * reserves.  reserves, rates: (m, 2); amp: (m,) (Curve's A(), not A n^n).  Curve's get_D Newton
+    balances y = rates * reserves.  reserves, rates: (m, 2); amp: (m,), the whitepaper amplification A (a contract's
+    A() / n^(n-1) = A() / 2; earlier versions of this docstring called it Curve's A(), which it is not).  Curve's get_D Newton
     iteration in fp64 on the balances in units of y0 + y1 (the invariant is homogeneous of degree 1), from D = y0 + y1
     down to the root (monotone: the cubic is convex there); a pool stops once a step
     moves D by at most 2 ulp.  Elementwise: a pool's D does not depend on the other pools of the call, so a subset
@@ -49,6 +52,59 @@ def stableswap_invariant(reserves, rates, amp) -> np.ndarray:
     return out * scale
 
 
+def stableswap_invariant_n(reserves, rates, amp) -> np.ndarray:
+    """Invariant D of n-coin StableSwap pools (n = 2..8, one n per call): the root of
+        A n^n sum(y) + D = A n^n D + D^(n+1) / (n^n prod(y)),     y = rates * reserves,
+    with A the whitepaper amplification (a contract's A() / n^(n-1)).  reserves, rates: (m, n); amp: (m,).  Curve's get_D
+    generalised: the Newton step D <- (Ann S + n D_P) D / ((Ann - 1) D + (n + 1) D_P), D_P = D^(n+1) / (n^n prod y),
+    Ann = A n^n, in fp64 on the balances in units of S = sum(y).  It starts from the upper bound
+    D0 = min(S, ((Ann + 1) S n^n prod y)^(1/(n+1))) (D_P <= Ann S + D <= (Ann + 1) S at the root), so an imbalanced
+    pool does not crawl down from S; Newton on this convex function then falls monotonically to the root.  A pool stops
+    once a step moves D by at most 2 ulp.  Elementwise, like stableswap_invariant.  Two-coin pools should go through
+    stableswap_invariant, whose arithmetic HostPools has always used (stableswap_invariant_any dispatches)."""
+    R = np.asarray(reserves, np.float64)
+    n = R.shape[-1]
+    y = R.reshape(-1, n) * np.asarray(rates, np.float64).reshape(-1, n)
+    ann = np.asarray(amp, np.float64).reshape(-1) * float(n ** n)
+    # every sum over the coins runs column by column in index order: numpy's row reductions take a different order
+    # for C- and F-ordered inputs (at n = 8), and HostPools and PoolStore.update_pools must get the same bits
+    colsum = lambda x: functools.reduce(lambda acc, j: acc + x[:, j], range(1, n), x[:, 0].copy())
+    scale = colsum(y)
+    with np.errstate(all="ignore"):
+        y = y / scale[:, None]                                            # units of S: nothing over- or underflows
+        S = colsum(y)
+        lg = (np.log(ann + 1.0) + np.log(S) + n * np.log(n) + colsum(np.log(y))) / (n + 1)
+        out = np.minimum(S, np.exp(lg) * (1.0 + 1e-12))
+        act = np.arange(len(S))
+        for _ in range(255):
+            if len(act) == 0:
+                break
+            d, a_, ya = out[act], ann[act], y[act]
+            dp = d.copy()
+            for j in range(n):
+                dp = dp * d / (n * ya[:, j])
+            dn = (a_ * S[act] + n * dp) * d / ((a_ - 1.0) * d + (n + 1) * dp)
+            out[act] = dn
+            act = act[~(np.abs(dn - d) <= 4.5e-16 * dn)]
+    return out * scale
+
+
+def stableswap_invariant_any(reserves, rates, amp) -> np.ndarray:
+    """D of StableSwap pools of one coin count: stableswap_invariant for two coins, stableswap_invariant_n for more"""
+    n = np.asarray(reserves).shape[-1]
+    return (stableswap_invariant if n == 2 else stableswap_invariant_n)(reserves, rates, amp)
+
+
+def _stable_groups(kind, pool_ptr):
+    """(n, pool ids, (m, n) CSR offsets) of the StableSwap pools, one entry per coin count"""
+    ss = np.nonzero(np.asarray(kind) == KIND_STABLESWAP_HOST)[0]
+    if len(ss) == 0:
+        return []
+    ptr = np.asarray(pool_ptr, np.int64)
+    ar = ptr[ss + 1] - ptr[ss]
+    return [(int(k), ss[ar == k], ptr[ss[ar == k]][:, None] + np.arange(k)) for k in np.unique(ar).tolist()]
+
+
 @dataclasses.dataclass
 class HostPools:
     """CSR problem data on the host (numpy)."""
@@ -68,10 +124,8 @@ class HostPools:
             self.amp = np.zeros(m)
         if self.inv is None:
             self.inv = np.zeros(m)
-            ss = np.nonzero(np.asarray(self.kind) == KIND_STABLESWAP_HOST)[0]
-            if len(ss):
-                off = np.asarray(self.pool_ptr)[ss][:, None] + np.arange(2)
-                self.inv[ss] = stableswap_invariant(self.reserves[off], self.weights[off], self.amp[ss])
+            for _, ss, off in _stable_groups(self.kind, self.pool_ptr):
+                self.inv[ss] = stableswap_invariant_any(self.reserves[off], self.weights[off], self.amp[ss])
 
     @property
     def m(self) -> int:
@@ -82,8 +136,10 @@ class HostPools:
         """From the reference's literals: local_indices / reserves / fees (arbitrage.py:6-28) plus
         which cvxpy atom constrains each pool (arbitrage.py:63-74): 'geomean' (with weights[i] = the
         ``p=`` vector), 'product' (cp.geo_mean on 2 tokens) or 'sum'.  Beyond the reference: 'bounded_product' (weights[i]
-        = the two virtual-reserve offsets) and 'stableswap' (weights[i] = (A, r0, r1): Curve's amplification A() and
-        rate multipliers, (A, 1, 1) for a plain pool)."""
+        = the two virtual-reserve offsets) and 'stableswap' (2..8 coins, weights[i] = (A, r_0, ..., r_{n-1}): the
+        whitepaper amplification A, which is a contract's A() / n^(n-1), and Curve's rate multipliers; (A, 1, 1, 1) for a
+        plain 3pool-like pool).  Earlier versions of this docstring called A Curve's A(); the math has always taken the
+        whitepaper A."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
@@ -110,10 +166,11 @@ class HostPools:
                 kd.append(KIND_BOUNDED_HOST); wts += list(o)
             elif kinds[i] == "stableswap":
                 p = None if (weights is None or weights[i] is None) else np.asarray(weights[i], float).reshape(-1)
-                if k != 2 or p is None or len(p) != 3:
-                    raise ValueError(f"pool {i}: stableswap needs 2 tokens and weights[i] = (A, r0, r1)")
+                if not 2 <= k <= STABLE_ARITY_MAX or p is None or len(p) != k + 1:
+                    raise ValueError(f"pool {i}: stableswap needs 2..{STABLE_ARITY_MAX} tokens and weights[i] = "
+                                     "(A, r_0, ..., r_{n-1})")
                 _check_stableswap(p[0], p[1:], reserves[i], f"pool {i}: ")
-                kd.append(KIND_STABLESWAP_HOST); wts += [float(p[1]), float(p[2])]; amp[i] = p[0]
+                kd.append(KIND_STABLESWAP_HOST); wts += [float(x) for x in p[1:]]; amp[i] = p[0]
             elif kinds[i] in ("geomean", "product"):
                 w = np.ones(k) if (weights is None or weights[i] is None) else np.asarray(weights[i], float)
                 if len(w) != k or np.any(w <= 0):
@@ -156,11 +213,9 @@ class HostPools:
             raise ValueError("fees (gamma) must lie in (0, 1]")
         if self.tok_idx.min(initial=0) < 0 or self.tok_idx.max(initial=0) >= self.n_tokens:
             raise ValueError("token index out of range")
-        ss = np.nonzero(np.asarray(self.kind) == KIND_STABLESWAP_HOST)[0]
-        if len(ss):
-            if np.any(np.diff(self.pool_ptr)[ss] != 2):
-                raise ValueError("stableswap pools must have 2 tokens")
-            off = self.pool_ptr[ss][:, None] + np.arange(2)
+        for k, ss, off in _stable_groups(self.kind, self.pool_ptr):
+            if not 2 <= k <= STABLE_ARITY_MAX:
+                raise ValueError(f"stableswap pools must have 2..{STABLE_ARITY_MAX} tokens")
             _check_stableswap(self.amp[ss], self.weights[off], self.reserves[off])
             D = np.asarray(self.inv, float)[ss]
             if not bool(np.all(np.isfinite(D) & (D > 0))):
@@ -168,10 +223,13 @@ class HostPools:
 
 
 def _check_stableswap(A, rates, reserves, where=""):
-    """The value rules of StableSwap pools: A finite in (0, AMP_MAX], rates finite and > 0, reserves finite and > 0."""
+    """The value rules of StableSwap pools of n coins (the last axis of rates): A finite, A > 0 and A n^n <= ANN_MAX
+    (A <= 1e7 at n = 2), rates finite and > 0, reserves finite and > 0."""
     A, r, R = np.asarray(A, float), np.asarray(rates, float), np.asarray(reserves, float)
-    if not bool(np.all((A > 0) & (A <= AMP_MAX))):
-        raise ValueError(f"{where}stableswap amplification A must be finite and in (0, {AMP_MAX:g}]")
+    n = r.shape[-1]
+    if not bool(np.all((A > 0) & (A * float(n ** n) <= ANN_MAX))):
+        raise ValueError(f"{where}stableswap amplification A must be finite, > 0 and A n^n <= {ANN_MAX:g} "
+                         f"(A <= {ANN_MAX / n ** n:g} for {n} coins)")
     if not bool(np.all(np.isfinite(r) & (r > 0))):
         raise ValueError(f"{where}stableswap rates must be finite and > 0")
     if not bool(np.all(np.isfinite(R) & (R > 0))):
@@ -317,9 +375,12 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         keys.append((_lib.KIND_BOUNDED, 2, np.nonzero(bp)[0]))
     ss = hp.kind == KIND_STABLESWAP_HOST
     if ss.any():
-        if np.any(ar[ss] != 2):
-            raise ValueError("stableswap pools must have 2 tokens")
-        keys.append((_lib.KIND_STABLESWAP, 2, np.nonzero(ss)[0]))
+        if np.any((ar[ss] < 2) | (ar[ss] > STABLE_ARITY_MAX)):
+            raise ValueError(f"stableswap pools must have 2..{STABLE_ARITY_MAX} tokens")
+        if np.any(ss & (ar == 2)):                  # two coins: the kind-4 bucket (k_eval_stable)
+            keys.append((_lib.KIND_STABLESWAP, 2, np.nonzero(ss & (ar == 2))[0]))
+        for k in np.unique(ar[ss & (ar > 2)]).tolist():  # more: one kind-5 bucket per coin count (k_eval_stable_n<K>)
+            keys.append((_lib.KIND_STABLESWAP_N, int(k), np.nonzero(ss & (ar == k))[0]))
     gm = (hp.kind == KIND_GEOMEAN_HOST) & ~is_cp
     for k in np.unique(ar[gm]).tolist():
         if k < 2 or k > 32:
@@ -374,7 +435,7 @@ class DeviceBucket:
             self.logrw = torch.as_tensor(_padded(np.log(R / W), self.stride, 0.0), **f64)
         if self.kind == _lib.KIND_BOUNDED:                 # the virtual-reserve offsets ride in the weights slot
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
-        if self.kind == _lib.KIND_STABLESWAP:              # rates in the weights slot, (A, D) in the two logrw slots
+        if self.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N):   # rates in the weights slot, (A, D) in two logrw rows
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
             AD = np.stack([hp.amp[spec.sel], hp.inv[spec.sel]])
             self.logrw = torch.as_tensor(_padded(AD, self.stride, 1.0), **f64)
@@ -406,8 +467,8 @@ class DeviceBucket:
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
         if R is not None:
             self.reserves[:, li] = torch.as_tensor(R, **f64)
-            if self.kind == _lib.KIND_STABLESWAP:
-                self.logrw[1, li] = torch.as_tensor(stableswap_invariant(R.T, W.T, amp), **f64)
+            if self.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N):
+                self.logrw[1, li] = torch.as_tensor(stableswap_invariant_any(R.T, W.T, amp), **f64)
             elif self.logrw is not None:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
         if gamma is not None:
@@ -426,7 +487,9 @@ class DeviceBucket:
             self.delta = torch.zeros((self.arity, self.stride), **f64)
             self.lam = torch.zeros((self.arity, self.stride), **f64)
         if hess and self.hcoef is None:
-            self.hcoef = torch.zeros(self.stride, **f64)
+            # n-coin StableSwap: one coefficient h_j per slot ([arity][stride]); every other kind: one per pool
+            self.hcoef = torch.zeros((self.arity, self.stride) if self.kind == _lib.KIND_STABLESWAP_N else self.stride,
+                                     **f64)
             self.hmask = torch.zeros(self.stride, dtype=torch.int32, device=self._device)
         return _lib.EvalOut(self.delta.data_ptr() if trades else None, self.lam.data_ptr() if trades else None,
                             self.hcoef.data_ptr() if hess else None, self.hmask.data_ptr() if hess else None)
@@ -909,11 +972,13 @@ class PoolStore:
         return sum(b.bytes_resident() for b in self.buckets)
 
     def algorithmic_bytes_per_eval(self) -> int:
-        """SURVEY.md section 8(d): 32 B per 2-token pool, 28k+12 per weighted pool, + nu, psi, arb."""
+        """SURVEY.md section 8(d): 32 B per 2-token pool, 28k+12 per weighted pool, 20k+24 per StableSwap pool (reserves,
+        token ids, rates, gamma, A, D), + nu, psi, arb."""
         n = 0
         for b in self.buckets:
             n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED
-                        else 64 if b.kind == _lib.KIND_STABLESWAP else 32)
+                        else 64 if b.kind == _lib.KIND_STABLESWAP
+                        else 20 * b.arity + 24 if b.kind == _lib.KIND_STABLESWAP_N else 32)
         return n + 16 * self.n_tokens + 8
 
     # -- the hot path --------------------------------------------------------------------------
@@ -1060,7 +1125,7 @@ class PoolStore:
         for b, l, R, g, rs, ids in plan:
             if not getattr(b, "blocked", False):
                 W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None) else None
-                amp = self._amp_host[ids] if b.kind == _lib.KIND_STABLESWAP else None
+                amp = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) else None
                 b.write_update(l, R, g, W, amp)
         torch.cuda.synchronize(self.device)
         return rebuilt

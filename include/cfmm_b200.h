@@ -13,7 +13,7 @@
  *   tok_idx [k][n_pools]  i32   local_indices  arbitrage.py:6-12   (replaces dense A_i, :42-48)
  *   gamma   [n_pools]     f64   fees[i]        arbitrage.py:22-28
  *   weights [k][n_pools]  f64   normalised p/sum(p) of cp.geo_mean(x, p=...)   arbitrage.py:65
- *   logrw   [k][n_pools]  f64   log(R/w), precomputed once (weighted pools); StableSwap: (A, D) per pool
+ *   logrw   [k][n_pools]  f64   log(R/w), precomputed once (weighted pools); StableSwap: (A, D) per pool ([2][n_pools])
  *   (StableSwap pools carry their rates in `weights`, bounded products their virtual-reserve offsets)
  *   theta_bar[2][n_pools] f64   constant-sum fills (multipliers of the kink), updated by the solver
  */
@@ -33,10 +33,19 @@ enum {
     CFMM_KIND_BOUNDED_PRODUCT = 3, /* sqrt((x1+o1)(x2+o2)) >= sqrt((R1+o1)(R2+o2)), x >= 0: constant product on virtual
                               reserves, one Uniswap-v3 tick range.  Not in the reference (a new atom for the cons list
                               of arbitrage.py:63-74); arity 2, the two offsets passed in `weights`                */
-    CFMM_KIND_STABLESWAP = 4 /* two-coin StableSwap (Curve): 4A(y0+y1) + D >= 4AD + D^3/(4 y0 y1), y_j = r_j x_j, where
+    CFMM_KIND_STABLESWAP = 4, /* two-coin StableSwap (Curve): 4A(y0+y1) + D >= 4AD + D^3/(4 y0 y1), y_j = r_j x_j, where
                               D = D(R) is the invariant of the current reserves.  Not in the reference; arity 2.
                               weights [2][stride] = the rates (r0, r1) > 0; logrw [2][stride] = per-pool constants:
-                              slot 0 = A (Curve's A(), not A n^n), slot 1 = D.  Smooth (no kink): no theta_bar       */
+                              slot 0 = A, slot 1 = D.  A is the whitepaper amplification (A n^n = 4A is the
+                              coefficient), which is a contract's A() / n^(n-1) = A() / 2; earlier versions of this
+                              header called it Curve's A(), which it is not.  Smooth (no kink): no theta_bar          */
+    CFMM_KIND_STABLESWAP_N = 5 /* n-coin StableSwap (Curve), arity n = 2..8 (3pool: n = 3):
+                              A n^n sum(y) + D >= A n^n D + D^(n+1) / (n^n prod y), y_j = r_j x_j, D = D(R); at n = 2
+                              this is CFMM_KIND_STABLESWAP.  weights [n][stride] = the rates; logrw [2][stride]: slot 0 =
+                              A (whitepaper, as kind 4), slot 1 = D.  cfmm_eval_out.hcoef is [n][stride]: the per-slot
+                              h_j of the pool's scaled Hessian Hs = C - (C1)(C1)'/(1'C1), C = diag(h^2) - h h'/(1+k)
+                              on its k traded slots (hmask), 0 on the others.  Arity 2 is accepted so both kinds can
+                              run the same pools; the Python layer sends only n >= 3 here                             */
 };
 
 enum {
@@ -51,15 +60,15 @@ enum {
 
 typedef struct cfmm_bucket {
     int32_t kind;          /* CFMM_KIND_*                                                */
-    int32_t arity;         /* tokens per pool: 2 for PRODUCT and SUM, 2..32 for GEOMEAN  */
+    int32_t arity;         /* tokens per pool: 2 for PRODUCT and SUM, 2..32 for GEOMEAN, 2..8 for STABLESWAP_N */
     int64_t n_pools;
     int64_t stride;        /* elements between consecutive slots (>= n_pools); the TMA-staged path needs
                               stride % 1024 == 0 and 16-byte aligned arrays, otherwise the LDG path runs */
     const double* reserves;
     const int32_t* tok_idx;
     const double* gamma;
-    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP rates */
-    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP (A, D) */
+    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates */
+    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D) */
     const double* theta_bar; /* SUM only     */
 } cfmm_bucket;
 
@@ -67,8 +76,9 @@ typedef struct cfmm_bucket {
 typedef struct cfmm_eval_out {
     double* delta;   /* [arity][n_pools]  = deltas[i].value    arbitrage.py:51, two-asset.py:97  */
     double* lambda;  /* [arity][n_pools]  = lambdas[i].value   arbitrage.py:52, two-asset.py:97  */
-    double* hcoef;   /* [n_pools] curvature coefficient of arb_i in log-price coordinates        */
-    uint32_t* hmask; /* [n_pools] GEOMEAN: bit j set iff token j is traded                      */
+    double* hcoef;   /* [n_pools] curvature coefficient of arb_i in log-price coordinates        *
+                      * (STABLESWAP_N: [arity][n_pools], one coefficient h_j per slot)          */
+    uint32_t* hmask; /* [n_pools] GEOMEAN, STABLESWAP_N: bit j set iff token j is traded        */
 } cfmm_eval_out;
 
 /*
@@ -314,6 +324,11 @@ int cfmm_batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const
  * cfmm_batch_solve keeps the occupancy it has without them.  Same arguments, limits and workspace. */
 int cfmm_batch_solve_stableswap(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
                                 void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_STABLESWAP pools of more than two coins (kind 4 in the CSR arrays,
+ * 2..8 coins; the two entry points above give their problems status 3).  A third kernel instance, so the other two keep
+ * their registers.  Same arguments, limits and workspace. */
+int cfmm_batch_solve_stableswap_n(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
+                                  void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
