@@ -106,7 +106,9 @@ def solve(local_indices, reserves, fees, kinds, weights=None, utility=None, n_to
     """Solve the routing problem the reference scripts pose.  `kinds[i]` in {'geomean','product','sum'}
     names the cvxpy atom on pool i (arbitrage.py:63-74); `weights[i]` is the geo_mean ``p=`` vector.  Two more kinds:
     'bounded_product' (weights[i] = virtual-reserve offsets) and 'stableswap' (weights[i] = (A, r_0, ..., r_{n-1}), a
-    Curve pool of 2..8 coins with the whitepaper A = A() / n^(n-1); see HostPools.from_lists)."""
+    Curve pool of 2..8 coins with the whitepaper A = A() / n^(n-1); see HostPools.from_lists).  And 'concentrated':
+    weights[i] = (price, bounds, liquidity), a whole Uniswap-v3 tick ladder as one pool, with reserves[i] = None (see
+    HostPools.from_lists and instances.v3_ladder)."""
     if utility is None:
         raise ValueError("utility is required: Arbitrage(c) | Liquidate(target, assets) | Swap(i, o, t)")
     if n_tokens is None:

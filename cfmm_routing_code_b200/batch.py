@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .pools import HostPools, KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
+from .pools import HostPools, KIND_CONCENTRATED_HOST, KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
 from .solver import default_nu0
 
 NTOK_MAX = 64      # cfmm_small::NTOK_MAX
@@ -56,6 +56,18 @@ class CsrStore:
             first = torch.as_tensor(np.asarray(hp.pool_ptr)[ss], device=dev)
             self.logrw[first] = torch.as_tensor(np.asarray(hp.amp, np.float64)[ss], device=dev)
             self.logrw[first + 1] = torch.as_tensor(np.asarray(hp.inv, np.float64)[ss], device=dev)
+        cl = np.nonzero(np.asarray(hp.kind) == KIND_CONCENTRATED_HOST)[0]
+        self.has_ladder = bool(len(cl))              # -> cfmm_batch_solve_concentrated (a fourth instance)
+        self.records = None
+        if len(cl):                                  # concentrated pools: (s, c) in the w slots, (first record, T) in logrw
+            first = torch.as_tensor(np.asarray(hp.pool_ptr)[cl], device=dev)
+            lp = np.asarray(hp.lad_ptr, np.int64)
+            sc = np.asarray(hp.lad_sc, np.float64)[cl]
+            self.w[first] = torch.as_tensor(sc[:, 0], device=dev)
+            self.w[first + 1] = torch.as_tensor(sc[:, 1], device=dev)
+            self.logrw[first] = torch.as_tensor(lp[cl].astype(np.float64), device=dev)
+            self.logrw[first + 1] = torch.as_tensor((lp[cl + 1] - lp[cl] - 1).astype(np.float64), device=dev)
+            self.records = torch.as_tensor(np.ascontiguousarray(hp.lad_rec, np.float64).reshape(-1), device=dev)
         self.gamma = torch.as_tensor(np.ascontiguousarray(hp.gamma, np.float64), device=dev)
         self.kind = torch.as_tensor(np.ascontiguousarray(hp.kind, np.uint8), device=dev)
         self.c_pools = _lib.CsrPools(self.n_tokens, self.m, self.nnz, self.pool_ptr.data_ptr(), self.tok.data_ptr(),
@@ -108,6 +120,11 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if store.has_ladder:
+        _lib.check(store.lib.cfmm_batch_solve_concentrated(C.byref(store.c_pools), store.records.data_ptr(),
+                                                           C.byref(batch), C.byref(prm), work.data_ptr(), st),
+                   "cfmm_batch_solve_concentrated")
+        return psi, stats, delta, lam
     entry = (store.lib.cfmm_batch_solve_stableswap_n if store.has_stableswap_n else
              store.lib.cfmm_batch_solve_stableswap if store.has_stableswap else store.lib.cfmm_batch_solve)
     _lib.check(entry(C.byref(store.c_pools), C.byref(batch), C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve")
@@ -169,12 +186,14 @@ def pack_problems(problems: Sequence):
     n = max(hp.n_tokens for hp, _ in problems)
     B = len(problems)
     ptr = [np.zeros(1, np.int64)]
+    lptr = [np.zeros(1, np.int64)]               # concentrated records: their per-pool offsets shift like pool_ptr
     ranges = np.empty((B, 2), np.int64)
     c = np.zeros((B, n)); a = np.zeros((B, n)); fl = np.full((B, n), 2, np.uint8); nu = np.ones((B, n))
     m0, off0, nnz_max = 0, 0, 0
     for p, (hp, u) in enumerate(problems):
         hp.validate()
         ptr.append(np.asarray(hp.pool_ptr[1:], np.int64) + off0)
+        lptr.append(np.asarray(hp.lad_ptr[1:], np.int64) + lptr[-1][-1])
         ranges[p] = (m0, m0 + hp.m)
         m0 += hp.m
         off0 += int(hp.pool_ptr[-1])
@@ -188,7 +207,9 @@ def pack_problems(problems: Sequence):
     cat = lambda name, dt: np.concatenate([np.asarray(getattr(hp, name), dt) for hp, _ in problems])
     merged = HostPools(n, np.concatenate(ptr), cat("tok_idx", np.int32), cat("reserves", np.float64),
                        cat("weights", np.float64), cat("gamma", np.float64), cat("kind", np.uint8),
-                       cat("amp", np.float64), cat("inv", np.float64))
+                       cat("amp", np.float64), cat("inv", np.float64), np.concatenate(lptr),
+                       np.concatenate([np.asarray(hp.lad_rec, np.float64).reshape(-1, 4) for hp, _ in problems]),
+                       np.concatenate([np.asarray(hp.lad_sc, np.float64).reshape(-1, 2) for hp, _ in problems]))
     return merged, ranges, c, a, fl, nu, nnz_max
 
 

@@ -5,15 +5,18 @@ import os
 import shutil
 import subprocess
 import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, os.environ.get("CFMM_LIB", "libcfmm_b200.so"))      # (CFMM_LIB: load / build an experiment variant)
-SOURCES = ["cfmm_kernels.cu", "cfmm_blocked.cu", "cfmm_layout.cu", "cfmm_persist.cu", "cfmm_solver.cu", "cfmm_allreduce.cu", "cfmm_small.cu"]
+SOURCES = ["cfmm_kernels.cu", "cfmm_blocked.cu", "cfmm_layout.cu", "cfmm_persist.cu", "cfmm_solver.cu", "cfmm_allreduce.cu",
+           "cfmm_small.cu", "cfmm_small_ladder.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
-    "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
+    "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
 
@@ -35,18 +38,35 @@ def needs_build() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
+    """Compile every translation unit to an object in parallel (each one is compiled whole, as a single nvcc call
+    would; ptxas runs single-threaded per unit, and the per-thread solver instances take it minutes), then link the
+    shared library.  The ptxas report of every unit, in SOURCES order, goes to build_ptxas.log."""
     if not force and not needs_build():
         return LIB
-    srcs = [os.path.join(CSRC, s) for s in SOURCES]
+    nvcc = _nvcc()
     extra = os.environ.get("CFMM_NVCC_EXTRA", "").split()
-    cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-I", os.path.join(ROOT, "include"), "-I", CSRC, "-o", LIB] + srcs
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if verbose or res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-    if res.returncode != 0:
-        raise RuntimeError("nvcc failed building libcfmm_b200.so")
+    inc = ["-I", os.path.join(ROOT, "include"), "-I", CSRC]
+    with tempfile.TemporaryDirectory(prefix="cfmm_build_") as tmp:
+        objs = [os.path.join(tmp, os.path.splitext(s)[0] + ".o") for s in SOURCES]
+
+        def compile_one(k):
+            cmd = [nvcc] + NVCC_FLAGS + extra + inc + ["-c", os.path.join(CSRC, SOURCES[k]), "-o", objs[k]]
+            return subprocess.run(cmd, capture_output=True, text=True)
+        with ThreadPoolExecutor(max_workers=max(1, min(len(SOURCES), os.cpu_count() or 1))) as ex:
+            results = list(ex.map(compile_one, range(len(SOURCES))))
+        log = "".join(r.stdout + r.stderr for r in results)
+        failed = [s for s, r in zip(SOURCES, results) if r.returncode != 0]
+        link = None
+        if not failed:
+            link = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC",
+                                   "-o", LIB] + objs, capture_output=True, text=True)
+            log += link.stdout + link.stderr
+        if verbose or failed or link.returncode != 0:
+            sys.stderr.write(log)
+        if failed or link.returncode != 0:
+            raise RuntimeError("nvcc failed building libcfmm_b200.so" + (f" ({', '.join(failed)})" if failed else ""))
     with open(os.path.join(HERE, "build_ptxas.log"), "w") as f:
-        f.write(res.stdout + res.stderr)
+        f.write(log)
     return LIB
 
 

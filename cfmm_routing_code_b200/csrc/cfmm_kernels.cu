@@ -9,7 +9,7 @@
 #include <math.h>
 
 #include "cfmm_dev.cuh"
-#include "cfmm_small.cuh"     // bounded_pair(): the bounded-liquidity pool math, shared with the per-thread solver
+#include "cfmm_small.cuh"     // bounded_pair(), ladder_pair(), ...: the per-pool math, shared with the per-thread solver
 
 namespace cfmm {
 std::atomic<long long> g_launches{0};
@@ -192,6 +192,40 @@ k_eval_stable(long long m, long long ld, int n_tokens, const double* __restrict_
         const double n0 = __ldg(nu + i0), n1 = __ldg(nu + i1);
         double D[2], L[2], h;
         cfmm_small::stableswap_pair(R[i], R[ld + i], rates[i], rates[ld + i], AD[i], AD[ld + i], gamma[i], n0, n1, D, L, h);
+        const double y0 = L[0] - D[0], y1 = L[1] - D[1];
+        if (TRADES) {
+            delta[i] = D[0]; delta[ld + i] = D[1];
+            lambda[i] = L[0]; lambda[ld + i] = L[1];
+        }
+        if (HESS) hcoef[i] = h;
+        if (y0 != 0.0) sc.add(i0, y0);
+        if (y1 != 0.0) sc.add(i1, y1);
+        acc += n0 * y0 + n1 * y1;
+    }
+    sc.flush(smem, n_tokens);
+    block_accumulate(acc, arb);
+}
+
+// concentrated liquidity (a whole tick ladder per pool): cfmm_small::ladder_pair, one thread per pool.  rec = the AoS
+// records (the bucket's weights), P [4][ld] = (s, c, first record, T) (the bucket's logrw).  The reserves are not read:
+// the flows come from the records.  A trade that stays in the current interval reads records c and c + 1; one that
+// crosses k bounds O(log k) more.
+template <typename Scatter, bool TRADES, bool HESS>
+__global__ void __launch_bounds__(kThreads)
+k_eval_ladder(long long m, long long ld, int n_tokens, const int* __restrict__ idx, const double* __restrict__ gamma,
+              const double* __restrict__ rec, const double* __restrict__ P, const double* __restrict__ nu, double* psi,
+              double* arb, double* delta, double* lambda, double* hcoef) {
+    extern __shared__ double smem[];
+    Scatter sc{psi};
+    sc.init(smem, n_tokens);
+    double acc = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        const int i0 = idx[i], i1 = idx[ld + i];
+        const double n0 = __ldg(nu + i0), n1 = __ldg(nu + i1);
+        double D[2], L[2], h;
+        cfmm_small::ladder_pair(rec + 4 * (long long)P[2 * ld + i], (long long)P[3 * ld + i], (long long)P[ld + i], P[i],
+                                gamma[i], n0, n1, D, L, h);
         const double y0 = L[0] - D[0], y1 = L[1] - D[1];
         if (TRADES) {
             delta[i] = D[0]; delta[ld + i] = D[1];
@@ -791,10 +825,33 @@ int dispatch_stable_n(const cfmm_bucket* b, int n_tokens, const double* nu, doub
     return launch_stable_n<K, false, false>(b, n_tokens, nu, psi, arb, out, st);
 }
 
+// concentrated buckets: the LDG path only, like the StableSwap kinds (the records are read by a data-dependent search)
+template <bool TRADES, bool HESS>
+int launch_ladder(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                  const cfmm_eval_out* out, cudaStream_t st) {
+    const long long m = b->n_pools;
+    double* delta = out ? out->delta : nullptr;
+    double* lambda = out ? out->lambda : nullptr;
+    double* hcoef = out ? out->hcoef : nullptr;
+    if (use_shared(n_tokens, m)) {
+        const size_t sm = (size_t)n_tokens * sizeof(double);
+        auto kern = k_eval_ladder<SharedScatter, TRADES, HESS>;
+        allow_smem(kern, sm);
+        kern<<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->tok_idx, b->gamma, b->weights, b->logrw, nu,
+                                                    psi, arb, delta, lambda, hcoef);
+    } else {
+        k_eval_ladder<GlobalScatter, TRADES, HESS><<<grid_for(m, 8), kThreads, 0, st>>>(
+            m, b->stride, n_tokens, b->tok_idx, b->gamma, b->weights, b->logrw, nu, psi, arb, delta, lambda, hcoef);
+    }
+    return check_launch();
+}
+
 template <int KIND, bool TRADES, bool HESS>
 int launch_kind(const cfmm_bucket* b, int n_tokens, const double* nu, double eps, double* psi, double* arb,
                 const cfmm_eval_out* out, cudaStream_t st) {
-    if constexpr (KIND == CFMM_KIND_STABLESWAP)
+    if constexpr (KIND == CFMM_KIND_CONCENTRATED)
+        return launch_ladder<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
+    else if constexpr (KIND == CFMM_KIND_STABLESWAP)
         return launch_stable<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
     else
         return launch_pair<KIND, TRADES, HESS>(b, n_tokens, nu, eps, psi, arb, out, st);
@@ -870,6 +927,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity < 2 || b->arity > 8) return CFMM_E_KIND;
             if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // rates; (A, D)
             break;
+        case CFMM_KIND_CONCENTRATED:
+            if (b->arity != 2) return CFMM_E_KIND;
+            if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // records; (s, c, first, T)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -899,6 +960,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_BOUNDED_PRODUCT>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP:
             return dispatch_pair<CFMM_KIND_STABLESWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_CONCENTRATED:
+            return dispatch_pair<CFMM_KIND_CONCENTRATED>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP_N:
             switch (b->arity) {
                 case 2: return dispatch_stable_n<2>(b, n_tokens, nu, psi, arb, out, st);

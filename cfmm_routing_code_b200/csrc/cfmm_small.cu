@@ -5,52 +5,11 @@
 // 3-5 tokens) by ONE kernel: thread p runs cfmm_small::solve_one on problem p.  Parallelism is over problems; the pool
 // data of a shared-pool sweep is read by all lanes at the same address (one broadcast transaction per warp), the
 // per-problem state is element-interleaved so lane accesses coalesce.
-#include "cfmm_dev.cuh"
-#include "cfmm_small.cuh"
+#include "cfmm_small_batch.cuh"
 
 using namespace cfmm;
 
 namespace {
-
-constexpr int kSmallThreads = 32;     // one warp per CTA: a sweep of 50 problems spreads over 2 SMs, 10^5 over all 132
-
-// LANES = 1: one problem per thread (throughput: 10^5 .. 10^6 problems).  LANES = 32: one problem per warp, the pool
-// loop of every evaluation split over the lanes (latency: a handful of problems, or problems with hundreds of pools);
-// each lane keeps its own copy of the state at work[(p * LANES + lane)], so `stride` counts lanes, not problems.
-// STABLE: also evaluate StableSwap pools (k_batch_solve_stable); without it such a pool makes its problem status 3.
-// STABLE_N: StableSwap pools of 2..8 coins (k_batch_solve_stable_n).
-template <int LANES, bool STABLE, bool STABLE_N = false>
-__device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, const cfmm_batch& B, const cfmm_small::Params& prm,
-                                                 int n, long long n_pools, double* work, long long stride) {
-    const long long gt = (long long)blockIdx.x * kSmallThreads + threadIdx.x;
-    const long long p = LANES == 1 ? gt : gt / LANES;
-    const int lane = LANES == 1 ? 0 : (int)(gt % LANES);
-    if (p >= B.n_problems) return;
-    cfmm_small::Problem Q;
-    Q.n = n;
-    Q.p0 = B.pool_range ? B.pool_range[2 * p] : 0;
-    Q.p1 = B.pool_range ? B.pool_range[2 * p + 1] : n_pools;
-    double* st = B.stats + 8 * p;
-    if (Q.p0 < 0 || Q.p1 > n_pools || Q.p0 > Q.p1) {
-        if (lane == 0) {
-            for (int x = 0; x < 7; ++x) st[x] = NAN;
-            st[7] = 3.0;
-        }
-        return;
-    }
-    Q.off0 = P.pool_ptr[Q.p0];
-    Q.c = B.c + p * n;
-    Q.a = B.a + p * n;
-    Q.flags = B.flags + p * n;
-    Q.delta = B.delta ? B.delta + p * B.trade_stride : nullptr;
-    Q.lam = B.lambda ? B.lambda + p * B.trade_stride : nullptr;
-    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE, STABLE_N>(P, Q, prm, B.nu + p * n, B.psi + p * n,
-                                                                               work + (LANES == 1 ? p : p * LANES + lane), stride, lane);
-    if (lane == 0) {
-        st[0] = r.value; st[1] = r.dual; st[2] = r.gap; st[3] = r.infeas; st[4] = r.err;
-        st[5] = (double)r.iters; st[6] = (double)r.evals; st[7] = (double)r.status;
-    }
-}
 
 template <int LANES>
 __global__ void __launch_bounds__(kSmallThreads)
@@ -77,11 +36,22 @@ k_batch_solve_stable_n(cfmm_small::Pools P, cfmm_batch B, cfmm_small::Params prm
     batch_solve_body<LANES, true, true>(P, B, prm, n, n_pools, work, stride);
 }
 
-int g_batch_lanes = 1;       // cfmm_set_batch_lanes: 1 | 32
-
-inline long long padded(long long b) { return (b + kSmallThreads - 1) / kSmallThreads * kSmallThreads; }
-
 }  // namespace
+
+int cfmm::g_batch_lanes = 1;
+
+int cfmm::batch_solve_check(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
+                            void* work) {
+    if (!pools || !batch || !prm) return CFMM_E_NULL;
+    if (batch->n_problems == 0) return CFMM_OK;
+    if (!pools->pool_ptr || !pools->tok_idx || !pools->reserves || !pools->weights || !pools->logrw || !pools->gamma ||
+        !pools->kind || !batch->c || !batch->a || !batch->flags || !batch->nu || !batch->psi || !batch->stats || !work)
+        return CFMM_E_NULL;
+    if ((batch->delta == nullptr) != (batch->lambda == nullptr)) return CFMM_E_NULL;
+    if (batch->n_problems < 0 || pools->n_pools < 0 || pools->nnz < 0 || batch->trade_stride < 0) return CFMM_E_SIZE;
+    if (pools->n_tokens < 1 || pools->n_tokens > cfmm_small::NTOK_MAX) return CFMM_E_KIND;
+    return CFMM_OK;
+}
 
 extern "C" int64_t cfmm_batch_solve_work_bytes(const cfmm_csr_pools* pools, int32_t n_problems, int64_t nnz_max) {
     if (!pools) return CFMM_E_NULL;
@@ -99,14 +69,8 @@ extern "C" int cfmm_set_batch_lanes(int32_t lanes) {
 namespace {
 int batch_solve(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm, void* work,
                 void* stream, int stable) {
-    if (!pools || !batch || !prm) return CFMM_E_NULL;
-    if (batch->n_problems == 0) return CFMM_OK;
-    if (!pools->pool_ptr || !pools->tok_idx || !pools->reserves || !pools->weights || !pools->logrw || !pools->gamma ||
-        !pools->kind || !batch->c || !batch->a || !batch->flags || !batch->nu || !batch->psi || !batch->stats || !work)
-        return CFMM_E_NULL;
-    if ((batch->delta == nullptr) != (batch->lambda == nullptr)) return CFMM_E_NULL;
-    if (batch->n_problems < 0 || pools->n_pools < 0 || pools->nnz < 0 || batch->trade_stride < 0) return CFMM_E_SIZE;
-    if (pools->n_tokens < 1 || pools->n_tokens > cfmm_small::NTOK_MAX) return CFMM_E_KIND;
+    const int rc = cfmm::batch_solve_check(pools, batch, prm, work);
+    if (rc != CFMM_OK || batch->n_problems == 0) return rc;
     cfmm_small::Pools P{pools->pool_ptr, pools->tok_idx, pools->reserves, pools->weights, pools->logrw, pools->gamma,
                         pools->kind};
     cfmm_small::Params q{prm->tol, prm->eps0, prm->eps_min, prm->eps_shrink, prm->floor_rel, prm->max_outer, prm->max_inner};
@@ -152,3 +116,4 @@ extern "C" int cfmm_batch_solve_stableswap_n(const cfmm_csr_pools* pools, const 
                                              const cfmm_batch_params* prm, void* work, void* stream) {
     return batch_solve(pools, batch, prm, work, stream, 2);
 }
+

@@ -102,6 +102,93 @@ CFMM_HD inline void bounded_pair(double R0, double R1, double o0, double o1, dou
     }
 }
 
+// Concentrated-liquidity pool (a whole Uniswap-v3 tick ladder): sqrt-price bounds b_0 < ... < b_T, liquidity L_k on
+// [b_k, b_{k+1}), current sqrt price s in [b_0, b_T] inside interval c (b_c <= s, c <= T - 1).  One record per bound,
+// rec[4k .. 4k+3] = {b_k, L_k, Y_k, X_k}: Y_k = sum_{j<k} L_j (b_{j+1} - b_j) (token 1 below b_k), X_k =
+// sum_{j>=k} L_j (1/b_j - 1/b_{j+1}) (token 0 above b_k), L_T = 0.  The trading set is the Minkowski sum of the
+// intervals' bounded-product sets, so at prices nu every interval moves to the same target sqrt price:
+//   tender 0 (the price falls) iff s* = sqrt(nu0 / (gamma nu1)) < s: s_f = max(s*, b_0), L_1 = y - Y(s_f),
+//     D_0 = (X(s_f) - x) / gamma;
+//   tender 1 (the price rises) iff s* = sqrt(gamma nu0 / nu1) > s: s_f = min(s*, b_T), D_1 = (Y(s_f) - y) / gamma,
+//     L_0 = x - X(s_f);
+//   hc = L(s_f) sqrt(nu0 nu1 / gamma) / 2, L(s_f) = the liquidity of the interval j the trade ends in.  At an exact
+//   bound s_f = b_j that is the interval above it, [b_j, b_{j+1}); past either end of the ladder (s* < b_0, s* >= b_T)
+//   and in an empty interval it is 0.  At T = 1 this is bounded_pair.
+// Precision: inside interval c the flows come from L_c and s - s_f (token 0: (s - s_f) / (s s_f), not a difference of
+// reciprocals), never from table differences;
+// across intervals they are the partial intervals at both ends plus the table difference over the whole intervals
+// between them, so the absolute error stays a few ulp of the reserves.  j is found by searching outward from c: c
+// first, then an exponential search toward s_f and a binary search, O(log |j - c|) record reads, fixed loop bounds.
+// Shared by the per-thread solver and k_eval_ladder (cfmm_kernels.cu).
+constexpr int64_t LADDER_T_MAX = int64_t(1) << 20;   // most intervals of one pool (pools.LADDER_T_MAX)
+constexpr int LADDER_SEARCH = 22;                    // >= log2(LADDER_T_MAX) + 2: the search loops' fixed bound
+
+// The largest j in [lo, hi) with b_j <= x, given b_lo <= x < b_hi (hi may be T + 1: b_{T+1} = +inf).
+CFMM_HD inline int64_t ladder_bisect(const double* rec, int64_t lo, int64_t hi, double x) {
+    for (int it = 0; it < LADDER_SEARCH; ++it) {
+        if (hi - lo <= 1) break;
+        const int64_t mid = lo + (hi - lo) / 2;
+        if (rec[4 * mid] <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+CFMM_HD inline void ladder_pair(const double* rec, int64_t T, int64_t c, double s, double gam, double n0, double n1,
+                                double* D, double* L, double& hc) {
+    D[0] = D[1] = L[0] = L[1] = 0.0;
+    hc = 0.0;
+    const double bc = rec[4 * c], Lc = rec[4 * c + 1], bc1 = rec[4 * (c + 1)];
+    const double hs = 0.5 * sqrt(n0 * n1 / gam);
+    const double sdn = sqrt(n0 / (gam * n1)), sup = sqrt(gam * n0 / n1);
+    if (sdn < s) {                                                     // tender token 0: the price falls to s_f
+        const double b0 = rec[0];
+        const double sf = fmax(sdn, b0);
+        int64_t j = c;
+        if (sf < bc) {                                                 // below interval c: exponential, then binary search
+            int64_t hi = c, lo = c;
+            for (int it = 0, step = 1; it < LADDER_SEARCH; ++it, step *= 2) {
+                lo = hi - step > 0 ? hi - step : 0;
+                if (rec[4 * lo] <= sf) break;
+                hi = lo;
+            }
+            j = ladder_bisect(rec, lo, hi, sf);
+        }
+        const double Lj = rec[4 * j + 1];
+        if (j == c) {
+            L[1] = Lc * (s - sf);
+            D[0] = Lc * ((s - sf) / (s * sf)) / gam;
+        } else {                                                       // partial c, whole intervals j+1 .. c-1, partial j
+            const double bj1 = rec[4 * (j + 1)];
+            L[1] = Lc * (s - bc) + (rec[4 * c + 2] - rec[4 * (j + 1) + 2]) + Lj * (bj1 - sf);
+            D[0] = (Lc * ((s - bc) / (s * bc)) + (rec[4 * (j + 1) + 3] - rec[4 * c + 3]) + Lj * ((bj1 - sf) / (sf * bj1))) / gam;
+        }
+        if (sdn >= b0) hc = Lj * hs;
+    } else if (sup > s) {                                              // tender token 1: the price rises to s_f
+        const double bT = rec[4 * T];
+        const double sf = fmin(sup, bT);
+        int64_t j = c;
+        if (sf >= bc1) {                                               // above interval c (j = T: past the top)
+            int64_t lo = c + 1, hi = c + 1;
+            for (int it = 0, step = 1; it < LADDER_SEARCH; ++it, step *= 2) {
+                hi = lo + step < T + 1 ? lo + step : T + 1;
+                if (hi > T || rec[4 * hi] > sf) break;
+                lo = hi;
+            }
+            j = ladder_bisect(rec, lo, hi, sf);
+        }
+        const double Lj = rec[4 * j + 1];                              // L_T = 0
+        if (j == c) {
+            D[1] = Lc * (sf - s) / gam;
+            L[0] = Lc * ((sf - s) / (s * sf));
+        } else {                                                       // partial c, whole intervals c+1 .. j-1, partial j
+            const double bj = rec[4 * j];
+            D[1] = (Lc * (bc1 - s) + (rec[4 * j + 2] - rec[4 * (c + 1) + 2]) + Lj * (sf - bj)) / gam;
+            L[0] = Lc * ((bc1 - s) / (s * bc1)) + (rec[4 * (c + 1) + 3] - rec[4 * j + 3]) + Lj * ((sf - bj) / (bj * sf));
+        }
+        hc = Lj * hs;
+    }
+}
+
 // Two-coin StableSwap (Curve) pool: scaled balances y_j = r_j x_j on the invariant
 //     4A (y0 + y1) + D = 4A D + D^3 / (4 y0 y1),        D = the invariant of the current reserves (precomputed),
 // worked in units of D (u_j = y_j / D, so 4A (u0 + u1) + 1 = 4A + 1 / (4 u0 u1)) so nothing overflows.  Along the curve
@@ -432,9 +519,13 @@ CFMM_UNROLL
 // STABLE_N (with STABLE): kind-4 pools of 2..KMAX coins, those of more than two through stableswap_n, whose k x k block
 // of Hs is added to the dense system; cfmm_batch_solve_stableswap_n runs this third instance.  Without it a kind-4 pool
 // of more than two coins makes its problem status 3.
-template <int LANES, bool STABLE = false, bool STABLE_N = false>
+// LADDER (with STABLE and STABLE_N): also concentrated pools (kind 6) through ladder_pair, their (s, c) in the pool's two
+// w slots, (first record, T) in its two logrw slots and the records in `rec`; cfmm_batch_solve_concentrated runs this
+// fourth instance.  The other instances give problems with such pools status 3.
+template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
-                               const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane) {
+                               const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane,
+                               const double* rec = nullptr) {
     const int n = Q.n;
     for (int j = 0; j < n; ++j) { lognu[j] = log(nu[j]); psi[j] = 0.0; }
     if (Hs) for (int e = 0; e < n * n; ++e) (*Hs)[e] = 0.0;
@@ -448,7 +539,16 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
         const int k = (int)(P.pool_ptr[i + 1] - off);
         const double gam = P.gamma[i];
         double D[KMAX], L[KMAX];
-        if (STABLE_N && P.kind[i] == 4 && k > 2) {                       // rates in w, (A, D) in logrw's first two slots
+        if (LADDER && P.kind[i] == 6) {                                   // (s, c) in w, (first record, T) in logrw
+            double hc = 0.0;
+            ladder_pair(rec + 4 * (int64_t)P.logrw[off], (int64_t)P.logrw[off + 1], (int64_t)P.w[off + 1], P.w[off], gam,
+                        nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
+            if (Hs && hc != 0.0) {
+                const int t0 = P.tok[off], t1 = P.tok[off + 1];
+                (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
+                (*Hs)[t0 * n + t1] -= hc; (*Hs)[t1 * n + t0] -= hc;
+            }
+        } else if (STABLE_N && P.kind[i] == 4 && k > 2) {                       // rates in w, (A, D) in logrw's first two slots
             double Rl[KMAX], rl[KMAX], nl[KMAX], hl[KMAX];
             for (int j = 0; j < KMAX; ++j) {
                 if (j < k) { Rl[j] = P.R[off + j]; rl[j] = P.w[off + j]; nl[j] = nu[P.tok[off + j]]; }
@@ -666,9 +766,10 @@ CFMM_HD inline int newton_direction(int n, uint64_t free_mask, const Vec& Hs, co
 CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL * n * n + (int64_t)n * (n + 1) + 2 * nnz; }
 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
-template <int LANES = 1, bool STABLE = false, bool STABLE_N = false>
+// rec: the concentrated pools' records (LADDER instance only).
+template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
-                               double* work, int64_t stride, int lane = 0) {
+                               double* work, int64_t stride, int lane = 0, const double* rec = nullptr) {
     const int n = Q.n;
     const int64_t nnz = P.pool_ptr[Q.p1] - Q.off0;
     int64_t e = 0;
@@ -686,8 +787,9 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int64_t o = P.pool_ptr[i];
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1;
-        bad = P.kind[i] > (STABLE ? 4 : 3) || k < 2 || k > KMAX ||
-              ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4)) && k != 2);
+        bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6)) || k < 2 || k > KMAX ||
+              ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
+                (LADDER && P.kind[i] == 6)) && k != 2);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
     if (bad) {
@@ -714,7 +816,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -760,7 +862,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -785,8 +887,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
+        evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -811,8 +913,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane));
+    evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

@@ -268,3 +268,151 @@ def v3_instance():
         weights=[o_a, o_b, o_c, None, [2, 1, 1]],
         market_value=[1.3, 1.0, 0.45],
     )
+
+
+# ------------------------------------------------------------------------------------------
+# concentrated liquidity: a whole Uniswap-v3 tick ladder as one pool (kind "concentrated")
+# ------------------------------------------------------------------------------------------
+def v3_ladder(sqrt_price_x96, ticks, liquidity_net, decimals0, decimals1):
+    """On-chain state of a Uniswap-v3 pool -> the (price, bounds, liquidity) of HostPools.from_lists' 'concentrated' kind,
+    in human token units (token 1 per token 0).  sqrt_price_x96: slot0's sqrtPriceX96; ticks: the initialised ticks
+    (any order); liquidity_net: each tick's liquidityNet (ints, as the contract stores them); decimals0/1: the tokens'
+    decimals.  price = (sqrt_price_x96 / 2^96)^2 10^(d0 - d1), bounds_k = 1.0001^tick_k 10^(d0 - d1) over the sorted
+    ticks, and the liquidity of [tick_k, tick_{k+1}) = the running sum of liquidity_net up to tick k, times
+    10^(-(d0 + d1) / 2).  Computed in 40-digit decimal and rounded once to f64."""
+    from decimal import Decimal, localcontext
+    order = np.argsort(np.asarray([int(t) for t in ticks], np.int64), kind="stable")
+    tk = [int(ticks[i]) for i in order]
+    net = [int(liquidity_net[i]) for i in order]
+    if len(tk) < 2 or len(set(tk)) != len(tk):
+        raise ValueError("v3_ladder needs at least two distinct initialised ticks")
+    with localcontext() as ctx:
+        ctx.prec = 40
+        dd = Decimal(10) ** (int(decimals0) - int(decimals1))
+        price = float(Decimal(int(sqrt_price_x96)) ** 2 / Decimal(2) ** 192 * dd)
+        bounds = [float(Decimal("1.0001") ** t * dd) for t in tk]
+        lscale = (Decimal(10) ** (-(int(decimals0) + int(decimals1)))).sqrt()
+        run, liq = 0, []
+        for x in net[:-1]:
+            run += x
+            if run < 0:
+                raise ValueError("liquidity_net sums to a negative liquidity")
+            liq.append(float(Decimal(run) * lscale))
+    return price, bounds, liq
+
+
+def ladder_ranges(hp):
+    """The same market with every concentrated pool written as its non-empty intervals, one bounded_product pool each:
+    the arithmetic of v3_position on the records' sqrt bounds (reserves L (1/s_k - 1/b_{k+1}), L (s_k - b_k) and offsets
+    L / b_{k+1}, L b_k with s_k = s clamped to [b_k, b_{k+1}]).  In exact arithmetic the two forms trade the same: the
+    ladder's trading set is the Minkowski sum of its intervals'.  Returns (HostPools, owner): owner[j] = the pool of hp
+    that pool j of the result comes from (other kinds are copied, in order)."""
+    from .pools import HostPools, KIND_BOUNDED_HOST, KIND_CONCENTRATED_HOST
+    ptr = np.asarray(hp.pool_ptr, np.int64)
+    lp = np.asarray(hp.lad_ptr, np.int64)
+    rec = np.asarray(hp.lad_rec, np.float64).reshape(-1, 4)
+    kind = np.asarray(hp.kind)
+    cl = kind == KIND_CONCENTRATED_HOST
+    # one entry per interval of every concentrated pool (the last record of each pool closes its ladder)
+    nrec = np.diff(lp)
+    owner_r = np.repeat(np.arange(hp.m), nrec)
+    last = np.zeros(len(rec), bool); last[lp[1:][nrec > 0] - 1] = True
+    iv = np.nonzero(~last & (rec[:, 1] > 0))[0]                      # non-empty intervals
+    o_iv = owner_r[iv]
+    L, b, b1 = rec[iv, 1], rec[iv, 0], rec[iv + 1, 0]
+    sk = np.minimum(np.maximum(np.asarray(hp.lad_sc, float)[o_iv, 0], b), b1)
+    Rr = np.stack([L * (1 / sk - 1 / b1), L * (sk - b)], 1)
+    Or = np.stack([L / b1, L * b], 1)
+    # pools of the result: every non-concentrated pool once, every concentrated pool as its intervals, in pool order
+    keep = np.nonzero(~cl)[0]
+    owner = np.concatenate([keep, o_iv])
+    order = np.argsort(owner, kind="stable")
+    owner = owner[order]
+    ar = np.where(cl, 2, np.diff(ptr))[owner]
+    new_ptr = np.concatenate([[0], np.cumsum(ar)]).astype(np.int64)
+    src_k = np.concatenate([keep, np.full(len(iv), -1)])[order]      # pool copied as it is, or -1: an interval
+    src_i = np.concatenate([np.full(len(keep), -1), np.arange(len(iv))])[order]
+    n = int(new_ptr[-1])
+    tok = np.zeros(n, np.int32); R = np.zeros(n); w = np.zeros(n)
+    kd = kind[owner].copy()
+    cp = src_k >= 0
+    within = np.arange(int(ar[cp].sum())) - np.repeat(np.cumsum(ar[cp]) - ar[cp], ar[cp])     # slot index in its pool
+    slots_new = np.repeat(new_ptr[:-1][cp], ar[cp]) + within
+    slots_old = np.repeat(ptr[src_k[cp]], ar[cp]) + within
+    tok[slots_new] = hp.tok_idx[slots_old]; R[slots_new] = hp.reserves[slots_old]; w[slots_new] = hp.weights[slots_old]
+    rng_ = ~cp
+    first = new_ptr[:-1][rng_]
+    ii = src_i[rng_]
+    tok[first] = hp.tok_idx[ptr[o_iv[ii]]]; tok[first + 1] = hp.tok_idx[ptr[o_iv[ii]] + 1]
+    R[first], R[first + 1] = Rr[ii, 0], Rr[ii, 1]
+    w[first], w[first + 1] = Or[ii, 0], Or[ii, 1]
+    kd[rng_] = KIND_BOUNDED_HOST
+    out = HostPools(hp.n_tokens, new_ptr, tok, R, w, np.asarray(hp.gamma, float)[owner], kd,
+                    np.asarray(hp.amp, float)[owner], np.asarray(hp.inv, float)[owner])
+    return out, owner
+
+
+def synth_concentrated_market(m, n_tokens, seed, T=(1, 64), frac_ladder=0.5, empty=0.1, mispricing=0.02):
+    """A market of concentrated pools (a tick ladder each) beside every other kind: m pools, a frac_ladder share of them
+    ladders on random token pairs with T intervals (an int, or a (lo, hi) range drawn log-uniformly) of geometric width
+    0.2 % .. 2 %, each empty with probability `empty`, the current price mispriced by `mispricing` and placed anywhere in
+    the ladder, a few pools past either end; the rest is synth_stable_n_market's mix (constant product, two- to four-coin
+    StableSwap) plus 5 % constant-sum pairs and 5 % bounded_product ranges.  Returns (HostPools, prices)."""
+    from .pools import (HostPools, KIND_BOUNDED_HOST, KIND_CONCENTRATED_HOST, KIND_SUM_HOST, ladder_records,
+                        ladder_state)
+    rng = np.random.default_rng(seed)
+    n_lad = int(round(frac_ladder * m))
+    n_sum = n_bnd = (m - n_lad) // 10
+    base = synth_stable_n_market(m - n_lad - n_sum - n_bnd, n_tokens, seed, mispricing=mispricing)
+    p = base.pop("prices")
+    ptr = [np.asarray(base["pool_ptr"], np.int64)]
+    tok, R, w = [base["tok_idx"]], [base["reserves"]], [base["weights"]]
+    g, kd, amp = [base["gamma"]], [base["kind"]], [base["amp"]]
+    def pairs(k):
+        a = rng.integers(0, n_tokens, k)
+        return a, (a + rng.integers(1, n_tokens, k)) % n_tokens
+    a, b = pairs(n_sum)                                                  # constant-sum pairs
+    tok.append(np.stack([a, b], 1).ravel()); R.append(np.exp(6.0 + rng.standard_normal(2 * n_sum)))
+    w.append(np.zeros(2 * n_sum)); g.append(_FEES[rng.integers(0, 3, n_sum)]); kd.append(np.full(n_sum, KIND_SUM_HOST))
+    amp.append(np.zeros(n_sum))
+    a, b = pairs(n_bnd)                                                  # single ranges
+    Lb = np.exp(6.0 + rng.standard_normal(n_bnd))
+    pr = p[a] / p[b] * np.exp(mispricing * rng.standard_normal(n_bnd))
+    sp, sa, sb = np.sqrt(pr), np.sqrt(pr * 0.9), np.sqrt(pr * 1.1)
+    tok.append(np.stack([a, b], 1).ravel()); R.append(np.stack([Lb * (1 / sp - 1 / sb), Lb * (sp - sa)], 1).ravel())
+    w.append(np.stack([Lb / sb, Lb * sa], 1).ravel()); g.append(_FEES[rng.integers(0, 3, n_bnd)])
+    kd.append(np.full(n_bnd, KIND_BOUNDED_HOST)); amp.append(np.zeros(n_bnd))
+    # ladders
+    if np.ndim(T) == 0:
+        Ts = np.full(n_lad, int(T))
+    else:
+        Ts = np.exp(rng.uniform(np.log(T[0]), np.log(T[1] + 1), n_lad)).astype(np.int64).clip(T[0], T[1])
+    a, b = pairs(n_lad)
+    price = p[a] / p[b] * np.exp(mispricing * rng.standard_normal(n_lad))
+    m0 = sum(len(x) for x in g)
+    recs = [None] * n_lad
+    for t in np.unique(Ts).tolist():
+        sel = np.nonzero(Ts == t)[0]
+        wd = np.exp(rng.uniform(np.log(0.002), np.log(0.02), len(sel)))
+        lo = np.log(price[sel]) - wd * t * rng.uniform(-0.05, 1.05, len(sel))        # some prices past either end
+        bounds = np.exp(lo[:, None] + wd[:, None] * np.arange(t + 1))
+        liq = np.exp(7.0 + rng.standard_normal((len(sel), t))) * (rng.random((len(sel), t)) >= empty)
+        liq[np.arange(len(sel)), rng.integers(0, t, len(sel))] = np.exp(7.0)            # never all empty
+        for x, r in zip(sel.tolist(), ladder_records(bounds, liq)):
+            recs[x] = r
+    tok.append(np.stack([a, b], 1).ravel()); w.append(np.zeros(2 * n_lad))
+    g.append(np.array([0.9995, 0.997, 0.99])[rng.integers(0, 3, n_lad)])
+    kd.append(np.full(n_lad, KIND_CONCENTRATED_HOST)); amp.append(np.zeros(n_lad))
+    M = m0 + n_lad
+    ar = np.concatenate([np.diff(ptr[0]), np.full(n_sum + n_bnd + n_lad, 2)])
+    lad_ptr = np.zeros(M + 1, np.int64)
+    lad_ptr[m0 + 1:] = np.cumsum(Ts + 1)
+    rec = np.concatenate(recs) if n_lad else np.zeros((0, 4))
+    ids = np.arange(m0, M)
+    s, c, x, y = ladder_state(lad_ptr, rec, ids, price)
+    R.append(np.stack([x, y], 1).ravel())
+    sc = np.zeros((M, 2)); sc[ids, 0], sc[ids, 1] = s, c
+    hp = HostPools(n_tokens, np.concatenate([[0], np.cumsum(ar)]).astype(np.int64),
+                   np.concatenate(tok).astype(np.int32), np.concatenate(R), np.concatenate(w), np.concatenate(g),
+                   np.concatenate(kd).astype(np.uint8), np.concatenate(amp), None, lad_ptr, rec, sc)
+    return hp, p

@@ -23,6 +23,76 @@ KIND_BOUNDED_HOST = 3   # constant product on virtual reserves (reserves + offse
 KIND_STABLESWAP_HOST = 4  # StableSwap (Curve), 2..8 coins; rates ride in `weights`, the amplification in HostPools.amp
 ANN_MAX = 4e7           # largest StableSwap coefficient A n^n accepted, any coin count (A <= 1e7 for two coins)
 STABLE_ARITY_MAX = 8    # most coins of a StableSwap pool
+KIND_CONCENTRATED_HOST = 6  # concentrated liquidity: a whole Uniswap-v3 tick ladder; records in HostPools.lad_rec
+LADDER_T_MAX = 1 << 20  # most intervals of one concentrated pool (cfmm_small::LADDER_T_MAX)
+
+
+def ladder_records(bounds, liquidity) -> np.ndarray:
+    """Records of concentrated pools with T intervals each: bounds (m, T + 1) prices (token 1 per token 0), strictly
+    increasing, and liquidity (m, T) >= 0.  Returns (m, T + 1, 4) f64 {b_k, L_k, Y_k, X_k}: the sqrt bound
+    b_k = sqrt(bounds_k), the liquidity of [b_k, b_{k+1}) (L_T = 0), the token 1 held below b_k,
+    Y_k = sum_{j<k} L_j (b_{j+1} - b_j), and the token 0 held above it, X_k = sum_{j>=k} L_j (1/b_j - 1/b_{j+1}).  The sums
+    run in extended precision (numpy longdouble) over the f64 b and L and are rounded once, so each entry is within about
+    an ulp of the exact sum of the stored b and L (for T up to a few thousand on x86-64)."""
+    b = np.sqrt(np.asarray(bounds, np.float64).reshape(len(bounds), -1))
+    Lq = np.asarray(liquidity, np.float64).reshape(len(b), -1)
+    m, T1 = b.shape
+    bl, Ll = b.astype(np.longdouble), Lq.astype(np.longdouble)
+    Y = np.zeros((m, T1), np.longdouble); X = np.zeros((m, T1), np.longdouble)
+    Y[:, 1:] = np.cumsum(Ll * (bl[:, 1:] - bl[:, :-1]), 1)
+    X[:, :-1] = np.cumsum((Ll * ((bl[:, 1:] - bl[:, :-1]) / (bl[:, :-1] * bl[:, 1:])))[:, ::-1], 1)[:, ::-1]
+    out = np.zeros((m, T1, 4))
+    out[:, :, 0] = b
+    out[:, :-1, 1] = Lq
+    out[:, :, 2] = Y.astype(np.float64)
+    out[:, :, 3] = X.astype(np.float64)
+    return out
+
+
+def ladder_state(lad_ptr, lad_rec, pool_ids, prices):
+    """The per-pool state of concentrated pools at new prices: (s, c, x, y), each (n,) f64.  s = sqrt(price) clamped to
+    [b_0, b_T] (the trading set is the same for every price beyond an end); c = the interval holding s (the largest c <= T - 1
+    with b_c <= s); the real reserves y = Y_c + L_c (s - b_c) and x = X_{c+1} + L_c (b_{c+1} - s) / (s b_{c+1}), evaluated
+    in extended precision and rounded once.  Elementwise: a pool's result does not depend on the other pools of the call,
+    so PoolStore.update_pools writes the same bits as a fresh HostPools."""
+    ids = np.asarray(pool_ids, np.int64).reshape(-1)
+    ptr = np.asarray(lad_ptr, np.int64)
+    rec = np.asarray(lad_rec, np.float64).reshape(-1, 4)
+    first = ptr[ids]
+    T = ptr[ids + 1] - first - 1
+    with np.errstate(invalid="ignore"):
+        s = np.minimum(np.maximum(np.sqrt(np.asarray(prices, np.float64).reshape(-1)), rec[first, 0]), rec[first + T, 0])
+    lo, hi = np.zeros(len(ids), np.int64), T - 1                     # the largest c in [lo, hi] with b_c <= s
+    for _ in range(24):
+        act = lo < hi
+        if not act.any():
+            break
+        mid = (lo + hi + 1) // 2
+        up = act & (rec[first + mid, 0] <= s)
+        lo = np.where(up, mid, lo)
+        hi = np.where(act & ~up, mid - 1, hi)
+    c = lo
+    bc, Lc, Yc = (rec[first + c, k].astype(np.longdouble) for k in (0, 1, 2))
+    bc1, Xc1 = (rec[first + c + 1, k].astype(np.longdouble) for k in (0, 3))
+    sl = s.astype(np.longdouble)
+    y = (Yc + Lc * (sl - bc)).astype(np.float64)
+    x = (Xc1 + Lc * ((bc1 - sl) / (sl * bc1))).astype(np.float64)
+    return s, c.astype(np.float64), x, y
+
+
+def _check_ladder(price, bounds, liquidity, where=""):
+    """The value rules of one concentrated pool given as (price, bounds, liquidity)"""
+    p, b, L = np.asarray(price, float), np.asarray(bounds, float).reshape(-1), np.asarray(liquidity, float).reshape(-1)
+    if p.size != 1 or not bool(np.isfinite(p) & (p > 0)):
+        raise ValueError(f"{where}concentrated price must be finite and > 0")
+    if len(b) < 2 or len(L) != len(b) - 1:
+        raise ValueError(f"{where}concentrated pools need T + 1 >= 2 bounds and T liquidities")
+    if len(L) > LADDER_T_MAX:
+        raise ValueError(f"{where}concentrated pools take at most {LADDER_T_MAX} intervals")
+    if not bool(np.all(np.isfinite(b) & (b > 0))) or not bool(np.all(b[1:] > b[:-1])):
+        raise ValueError(f"{where}concentrated bounds must be finite, > 0 and strictly increasing")
+    if not bool(np.all(np.isfinite(L) & (L >= 0))) or not bool(np.any(L > 0)):
+        raise ValueError(f"{where}concentrated liquidity must be finite, >= 0 and not all zero")
 
 
 def stableswap_invariant(reserves, rates, amp) -> np.ndarray:
@@ -117,9 +187,21 @@ class HostPools:
     kind: np.ndarray       # uint8 [m]
     amp: Optional[np.ndarray] = None   # f64 [m]  StableSwap amplification A, 0 on other kinds (None: all zero)
     inv: Optional[np.ndarray] = None   # f64 [m]  StableSwap invariant D of the reserves, 0 on other kinds (None: computed)
+    # concentrated pools (kind 6): pool i's T + 1 records are lad_rec[lad_ptr[i]:lad_ptr[i+1]] (none on other kinds),
+    # {b_k, L_k, Y_k, X_k} as ladder_records; lad_sc[i] = (s, c), the current sqrt price and its interval (ladder_state).
+    # Their reserves are the real (x, y) at s; their weights are 0.  None: no concentrated pools.
+    lad_ptr: Optional[np.ndarray] = None   # int64 [m+1]
+    lad_rec: Optional[np.ndarray] = None   # f64 [n_records, 4]
+    lad_sc: Optional[np.ndarray] = None    # f64 [m, 2]
 
     def __post_init__(self):
         m = len(self.gamma)
+        if self.lad_ptr is None:
+            self.lad_ptr = np.zeros(m + 1, np.int64)
+        if self.lad_rec is None:
+            self.lad_rec = np.zeros((0, 4))
+        if self.lad_sc is None:
+            self.lad_sc = np.zeros((m, 2))
         if self.amp is None:
             self.amp = np.zeros(m)
         if self.inv is None:
@@ -139,16 +221,33 @@ class HostPools:
         = the two virtual-reserve offsets) and 'stableswap' (2..8 coins, weights[i] = (A, r_0, ..., r_{n-1}): the
         whitepaper amplification A, which is a contract's A() / n^(n-1), and Curve's rate multipliers; (A, 1, 1, 1) for a
         plain 3pool-like pool).  Earlier versions of this docstring called A Curve's A(); the math has always taken the
-        whitepaper A."""
+        whitepaper A.  And 'concentrated' (a whole Uniswap-v3 tick ladder as one pool): weights[i] = (price, bounds,
+        liquidity) with the current price and the T + 1 price bounds in token 1 per token 0 (the caller's token units;
+        instances.v3_ladder converts on-chain state), T >= 1 liquidities >= 0 (not all 0), at most LADDER_T_MAX; reserves[i]
+        must be None: the real reserves are derived (ladder_state)."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
         ptr = [0]; idx: List[int] = []; res: List[float] = []; wts: List[float] = []; kd: List[int] = []
         amp = np.zeros(m)
+        lad = {}                                         # concentrated pool -> its records and price
         for i, l in enumerate(local_indices):
             k = len(l)
-            if len(reserves[i]) != k:
-                raise ValueError(f"pool {i}: {len(reserves[i])} reserves for {k} tokens")
+            if kinds[i] == "concentrated":
+                if k != 2 or len(set(int(t) for t in l)) != 2:
+                    raise ValueError(f"pool {i}: concentrated pools need 2 distinct tokens")
+                if reserves[i] is not None:
+                    raise ValueError(f"pool {i}: a concentrated pool's reserves[i] must be None (they are derived)")
+                if weights is None or weights[i] is None or len(weights[i]) != 3:
+                    raise ValueError(f"pool {i}: concentrated needs weights[i] = (price, bounds, liquidity)")
+                price, bounds, liq = weights[i]
+                _check_ladder(price, bounds, liq, f"pool {i}: ")
+                lad[i] = (float(price), ladder_records(np.asarray(bounds, float)[None, :], np.asarray(liq, float)[None, :])[0])
+                ptr.append(ptr[-1] + 2); idx += [int(t) for t in l]; res += [0.0, 0.0]; wts += [0.0, 0.0]
+                kd.append(KIND_CONCENTRATED_HOST)
+                continue
+            if reserves[i] is None or len(reserves[i]) != k:
+                raise ValueError(f"pool {i}: {0 if reserves[i] is None else len(reserves[i])} reserves for {k} tokens")
             if len(set(int(t) for t in l)) != k:
                 raise ValueError(f"pool {i}: repeated token in local_indices")
             ptr.append(ptr[-1] + k)
@@ -178,9 +277,24 @@ class HostPools:
                 kd.append(KIND_GEOMEAN_HOST); wts += list(w / w.sum())
             else:
                 raise ValueError(f"pool {i}: unknown kind {kinds[i]!r}")
+        res = np.asarray(res, np.float64)
+        lad_ptr = np.zeros(m + 1, np.int64); lad_sc = np.zeros((m, 2)); recs = []
+        if lad:
+            cnt = np.zeros(m, np.int64)
+            for i, (_, r) in lad.items():
+                cnt[i] = len(r)
+            lad_ptr[1:] = np.cumsum(cnt)
+            recs = [lad[i][1] for i in sorted(lad)]
+            ids = np.asarray(sorted(lad), np.int64)
+            rec = np.concatenate(recs)
+            sv, cv, x, y = ladder_state(lad_ptr, rec, ids, [lad[i][0] for i in ids.tolist()])
+            lad_sc[ids, 0], lad_sc[ids, 1] = sv, cv
+            first = np.asarray(ptr, np.int64)[ids]
+            res[first], res[first + 1] = x, y
         return HostPools(int(n_tokens), np.asarray(ptr, np.int64), np.asarray(idx, np.int32),
-                         np.asarray(res, np.float64), np.asarray(wts, np.float64),
-                         np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp)
+                         res, np.asarray(wts, np.float64),
+                         np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp, None, lad_ptr,
+                         np.concatenate(recs) if recs else None, lad_sc)
 
     @staticmethod
     def from_pairs(n_tokens, idx, reserves, gamma) -> "HostPools":
@@ -204,11 +318,15 @@ class HostPools:
         return self
 
     def validate(self):
-        slot_kind = np.repeat(np.asarray(self.kind), np.diff(self.pool_ptr)) if np.any(self.kind == KIND_BOUNDED_HOST) else None
+        slot_kind = np.repeat(np.asarray(self.kind), np.diff(self.pool_ptr)) if \
+            np.any((self.kind == KIND_BOUNDED_HOST) | (self.kind == KIND_CONCENTRATED_HOST)) else None
         virt = self.reserves if slot_kind is None else self.reserves + np.where(slot_kind == KIND_BOUNDED_HOST, self.weights, 0.0)
-        lo_ok = np.all(self.reserves > 0) if slot_kind is None else np.all(self.reserves >= 0) and np.all(virt > 0)
+        lo_ok = np.all(self.reserves > 0) if slot_kind is None else np.all(self.reserves >= 0) and \
+            np.all((virt > 0) | (slot_kind == KIND_CONCENTRATED_HOST))
         if not lo_ok or not np.all(np.isfinite(self.reserves)):
-            raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves)")
+            raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves; "
+                             "concentrated: >= 0)")
+        self._validate_ladders()
         if np.any(self.gamma <= 0) or np.any(self.gamma > 1):
             raise ValueError("fees (gamma) must lie in (0, 1]")
         if self.tok_idx.min(initial=0) < 0 or self.tok_idx.max(initial=0) >= self.n_tokens:
@@ -220,6 +338,45 @@ class HostPools:
             D = np.asarray(self.inv, float)[ss]
             if not bool(np.all(np.isfinite(D) & (D > 0))):
                 raise ValueError("stableswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
+
+
+    def _validate_ladders(self):
+        """The rules of concentrated pools on the CSR form: arity 2; T + 1 records, 1 <= T <= LADDER_T_MAX, none on other
+        kinds; bounds finite, > 0, strictly increasing; liquidity finite, >= 0, not all 0, L_T = 0; Y, X finite; (s, c) a
+        state of ladder_state."""
+        kind, m = np.asarray(self.kind), self.m
+        ptr = np.asarray(self.lad_ptr, np.int64)
+        rec = np.asarray(self.lad_rec, np.float64).reshape(-1, 4)
+        if len(ptr) != m + 1 or ptr[0] != 0 or np.any(np.diff(ptr) < 0) or ptr[-1] != len(rec):
+            raise ValueError("lad_ptr must be a CSR pointer of m + 1 entries over lad_rec")
+        cl = kind == KIND_CONCENTRATED_HOST
+        cnt = np.diff(ptr)
+        if np.any(cnt[~cl] != 0) or np.any((cnt[cl] < 2) | (cnt[cl] > LADDER_T_MAX + 1)):
+            raise ValueError(f"concentrated pools need 1..{LADDER_T_MAX} intervals (T + 1 records); other kinds none")
+        if not cl.any():
+            return
+        ids = np.nonzero(cl)[0]
+        if np.any(np.diff(self.pool_ptr)[ids] != 2):
+            raise ValueError("concentrated pools must have 2 tokens")
+        owner = np.repeat(np.arange(m), cnt)
+        last = np.zeros(len(rec), bool); last[ptr[ids + 1] - 1] = True
+        b, L = rec[:, 0], rec[:, 1]
+        inc = np.ones(len(rec), bool); inc[1:] = (b[1:] > b[:-1]) | (owner[1:] != owner[:-1])
+        if not (np.all(np.isfinite(b) & (b > 0)) and np.all(inc)):
+            raise ValueError("concentrated bounds must be finite, > 0 and strictly increasing")
+        if not (np.all(np.isfinite(L) & (L >= 0)) and np.all(L[last] == 0)):
+            raise ValueError("concentrated liquidity must be finite and >= 0 (0 at the last bound)")
+        if not np.all(np.bincount(owner, weights=(L > 0).astype(float), minlength=m)[ids] > 0):
+            raise ValueError("concentrated liquidity must not be all zero")
+        if not np.all(np.isfinite(rec[:, 2:])):
+            raise ValueError("concentrated records must be finite (token amounts out of fp64 range?)")
+        s, c = np.asarray(self.lad_sc, float)[ids, 0], np.asarray(self.lad_sc, float)[ids, 1]
+        T = cnt[ids] - 1
+        ok = np.isfinite(s) & (s >= rec[ptr[ids], 0]) & (s <= rec[ptr[ids] + T, 0]) & (c == np.floor(c)) & (c >= 0) & (c < T)
+        ci = np.where(ok, c, 0).astype(np.int64)
+        ok &= (rec[ptr[ids] + ci, 0] <= s) & ((rec[ptr[ids] + ci + 1, 0] > s) | (ci == T - 1))
+        if not bool(np.all(ok)):
+            raise ValueError("concentrated (s, c): s must lie in [b_0, b_T] and c be its interval")
 
 
 def _check_stableswap(A, rates, reserves, where=""):
@@ -244,14 +401,17 @@ class PoolUpdate:
     slots: np.ndarray                # int64 [nnz] CSR offsets of the updated pools' slots, pool by pool, in slot order
     reserves: Optional[np.ndarray]   # f64 [nnz] new reserves at `slots`, or None
     gamma: Optional[np.ndarray]      # f64 [n] new fees, or None
+    prices: Optional[np.ndarray] = None   # f64 [n] new prices of concentrated pools, or None
 
 
 def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarray, pool_ids, reserves=None,
-                      fees=None) -> PoolUpdate:
+                      fees=None, prices=None) -> PoolUpdate:
     """Host checks of PoolStore.update_pools, on the problem's CSR arrays (pool_ptr, kind, weights as in HostPools).
     pool_ids: global pool indices, distinct and in range; reserves[k]: the new reserve vector of pool pool_ids[k] with the
     pool's arity (a row of the reference's `reserves` literal; an (n, k) array when all pools have arity k); fees[k]: its
     new gamma.  The values must pass the rules of HostPools.validate (bounded_product pools with their own offsets).
+    prices[k]: the new price (token 1 per token 0) of pool pool_ids[k], which must then be concentrated; a concentrated pool
+    takes no reserves (they are derived from its price).
     Raises ValueError; returns the update with the reserves flattened into the pools' CSR slot order."""
     m = len(pool_ptr) - 1
     ids = np.asarray(pool_ids)
@@ -259,10 +419,22 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
         raise ValueError("pool_ids must be a 1-d sequence of integer pool indices")
     ids = ids.astype(np.int64)
     n = len(ids)
-    if reserves is None and fees is None:
-        raise ValueError("nothing to update: give reserves, fees or both")
+    if reserves is None and fees is None and prices is None:
+        raise ValueError("nothing to update: give reserves, fees, prices or several")
     if n and (ids.min() < 0 or ids.max() >= m):
         raise ValueError(f"pool id out of range [0, {m})")
+    conc = np.asarray(kind)[ids] == KIND_CONCENTRATED_HOST
+    if reserves is not None and conc.any():
+        raise ValueError("concentrated pools take prices=, not reserves= (their reserves are derived from the price)")
+    pr = None
+    if prices is not None:
+        pr = np.ascontiguousarray(prices, np.float64).reshape(-1)
+        if len(pr) != n:
+            raise ValueError("prices: one per pool")
+        if not bool(np.all(conc)):
+            raise ValueError("prices= applies to concentrated pools only")
+        if not bool(np.all(np.isfinite(pr) & (pr > 0))):
+            raise ValueError("concentrated prices must be finite and > 0")
     srt = np.sort(ids)                                   # (np.unique hashes: 20x slower at 100k ids)
     if bool(np.any(srt[1:] == srt[:-1])):
         raise ValueError("repeated pool id")
@@ -302,7 +474,7 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             raise ValueError("fees: one per pool")
         if not bool(np.all((g > 0) & (g <= 1))):
             raise ValueError("fees (gamma) must lie in (0, 1]")
-    return PoolUpdate(ids, first, slots, R, g)
+    return PoolUpdate(ids, first, slots, R, g, pr)
 
 
 class BucketSpec:
@@ -381,6 +553,11 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
             keys.append((_lib.KIND_STABLESWAP, 2, np.nonzero(ss & (ar == 2))[0]))
         for k in np.unique(ar[ss & (ar > 2)]).tolist():  # more: one kind-5 bucket per coin count (k_eval_stable_n<K>)
             keys.append((_lib.KIND_STABLESWAP_N, int(k), np.nonzero(ss & (ar == k))[0]))
+    cl = hp.kind == KIND_CONCENTRATED_HOST
+    if cl.any():
+        if np.any(ar[cl] != 2):
+            raise ValueError("concentrated pools must have 2 tokens")
+        keys.append((_lib.KIND_CONCENTRATED, 2, np.nonzero(cl)[0]))
     gm = (hp.kind == KIND_GEOMEAN_HOST) & ~is_cp
     for k in np.unique(ar[gm]).tolist():
         if k < 2 or k > 32:
@@ -439,6 +616,16 @@ class DeviceBucket:
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
             AD = np.stack([hp.amp[spec.sel], hp.inv[spec.sel]])
             self.logrw = torch.as_tensor(_padded(AD, self.stride, 1.0), **f64)
+        if self.kind == _lib.KIND_CONCENTRATED:            # this bucket's records in the weights slot, (s, c, first, T) in logrw
+            sel = spec.sel
+            first = np.asarray(hp.lad_ptr, np.int64)[sel]
+            cnt = np.asarray(hp.lad_ptr, np.int64)[sel + 1] - first
+            loc = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
+            gather = np.repeat(first - loc, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
+            self.weights = torch.as_tensor(np.ascontiguousarray(np.asarray(hp.lad_rec, np.float64)[gather]).reshape(-1), **f64)
+            sc = np.asarray(hp.lad_sc, np.float64)[sel]
+            P = np.stack([sc[:, 0], sc[:, 1], loc.astype(np.float64), (cnt - 1).astype(np.float64)])
+            self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
         if self.kind == _lib.KIND_SUM:
             self.theta_bar = torch.zeros((2, self.stride), **f64)
         self.delta = self.lam = self.hcoef = self.hmask = None
@@ -459,17 +646,20 @@ class DeviceBucket:
         return self.spec.off
 
     def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
-                     W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None):
+                     W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None, sc: Optional[np.ndarray] = None):
         """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
         Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__;
-        StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,)."""
+        StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,);
+        concentrated pools get their new (s, c) from sc (2, n), with R their derived reserves (ladder_state)."""
         f64 = dict(dtype=torch.float64, device=self._device)
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
+        if sc is not None:
+            self.logrw[:2, li] = torch.as_tensor(sc, **f64)
         if R is not None:
             self.reserves[:, li] = torch.as_tensor(R, **f64)
             if self.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N):
                 self.logrw[1, li] = torch.as_tensor(stableswap_invariant_any(R.T, W.T, amp), **f64)
-            elif self.logrw is not None:
+            elif self.kind == _lib.KIND_GEOMEAN:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
         if gamma is not None:
             self.gamma[li] = torch.as_tensor(gamma, **f64)
@@ -915,6 +1105,7 @@ class PoolStore:
         self._tok_idx_host = hp.tok_idx
         self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets / rates
         self._amp_host = hp.amp                                          # StableSwap amplification (structure too)
+        self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records (structure)
         self._where = None                                               # pool -> (bucket, position): update_pools
         self.rank, self.world = rank, world
         self.buckets = []
@@ -973,10 +1164,13 @@ class PoolStore:
 
     def algorithmic_bytes_per_eval(self) -> int:
         """SURVEY.md section 8(d): 32 B per 2-token pool, 28k+12 per weighted pool, 20k+24 per StableSwap pool (reserves,
-        token ids, rates, gamma, A, D), + nu, psi, arb."""
+        token ids, rates, gamma, A, D), 80 B per concentrated pool (token ids, gamma, (s, c, first record, T), and the b_c,
+        L_c, b_{c+1} and end bound the kernel reads for a trade inside the current interval; one that crosses bounds
+        reads O(log) records more), + nu, psi, arb."""
         n = 0
         for b in self.buckets:
             n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED
+                        else 80 if b.kind == _lib.KIND_CONCENTRATED
                         else 64 if b.kind == _lib.KIND_STABLESWAP
                         else 20 * b.arity + 24 if b.kind == _lib.KIND_STABLESWAP_N else 32)
         return n + 16 * self.n_tokens + 8
@@ -1087,14 +1281,17 @@ class PoolStore:
             self._where = (bi, loc)
         return self._where
 
-    def update_pools(self, pool_ids, reserves=None, fees=None):
+    def update_pools(self, pool_ids, reserves=None, fees=None, prices=None):
         """Set new reserves and / or fees of some pools in place: the store then equals, bit for bit, a PoolStore built
         from the updated host data, without re-uploading the pools or rebuilding the blocked layout (which depends on the
         token ids only).  pool_ids: global pool indices (the order of the problem's local_indices); reserves[k]: the new
         reserve vector of pool pool_ids[k], with the pool's arity (an (n, 2) array for pairs); fees[k]: its new gamma in
         (0, 1].  At least one of reserves / fees.  Kinds, tokens, weights, bounded_product offsets and StableSwap
         amplifications and rates cannot change (they are structure: build a new store, e.g. for a ramp of A); a StableSwap
-        pool's invariant D is recomputed from its new reserves, as HostPools does.
+        pool's invariant D is recomputed from its new reserves, as HostPools does.  Concentrated pools take prices=
+        (prices[k]: the new price of pool pool_ids[k], token 1 per token 0) instead of reserves=, which raises for them:
+        their (s, c) and real reserves are recomputed with ladder_state, the function HostPools uses, and their records
+        (bounds and liquidity, i.e. mints and burns) are structure.
 
         All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.validate) raise
         ValueError before anything is written, and so does an entry the device check of the blocked bucket rejects.
@@ -1105,7 +1302,7 @@ class PoolStore:
         A new block of the same market is then re-solved warm from the previous prices:
             store.update_pools(ids, reserves=new_R, fees=new_gamma)
             res = solve_pools(hp, utility, store=store, nu0=res.nu)"""
-        u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees)
+        u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees, prices)
         bi, loc = self._pool_map()
         owner = bi[u.ids]
         plan = []
@@ -1116,17 +1313,21 @@ class PoolStore:
             rs = u.ptr[e][None, :] + np.arange(b.arity)[:, None]          # (arity, n) indices into the update's slots
             R = None if u.reserves is None else u.reserves[rs]
             g = None if u.gamma is None else u.gamma[e]
-            plan.append((b, loc[u.ids[e]], R, g, rs, u.ids[e]))
+            sc = None
+            if u.prices is not None:                 # concentrated pools only (checked): state and reserves at the price
+                s, c, x, y = ladder_state(self._lad_host[0], self._lad_host[1], u.ids[e], u.prices[e])
+                sc, R = np.stack([s, c]), np.stack([x, y])
+            plan.append((b, loc[u.ids[e]], R, g, rs, u.ids[e], sc))
         # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
         rebuilt = 0
-        for b, l, R, g, _, _ in plan:
+        for b, l, R, g, _, _, _ in plan:
             if getattr(b, "blocked", False):
                 rebuilt += b.write_update(self.lib, l, R, g, self._stream())
-        for b, l, R, g, rs, ids in plan:
+        for b, l, R, g, rs, ids, sc in plan:
             if not getattr(b, "blocked", False):
                 W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None) else None
                 amp = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) else None
-                b.write_update(l, R, g, W, amp)
+                b.write_update(l, R, g, W, amp, sc)
         torch.cuda.synchronize(self.device)
         return rebuilt
 

@@ -14,7 +14,8 @@
  *   gamma   [n_pools]     f64   fees[i]        arbitrage.py:22-28
  *   weights [k][n_pools]  f64   normalised p/sum(p) of cp.geo_mean(x, p=...)   arbitrage.py:65
  *   logrw   [k][n_pools]  f64   log(R/w), precomputed once (weighted pools); StableSwap: (A, D) per pool ([2][n_pools])
- *   (StableSwap pools carry their rates in `weights`, bounded products their virtual-reserve offsets)
+ *   (StableSwap pools carry their rates in `weights`, bounded products their virtual-reserve offsets, concentrated
+ *   pools their records; see CFMM_KIND_CONCENTRATED)
  *   theta_bar[2][n_pools] f64   constant-sum fills (multipliers of the kink), updated by the solver
  */
 #ifndef CFMM_B200_H
@@ -39,13 +40,25 @@ enum {
                               slot 0 = A, slot 1 = D.  A is the whitepaper amplification (A n^n = 4A is the
                               coefficient), which is a contract's A() / n^(n-1) = A() / 2; earlier versions of this
                               header called it Curve's A(), which it is not.  Smooth (no kink): no theta_bar          */
-    CFMM_KIND_STABLESWAP_N = 5 /* n-coin StableSwap (Curve), arity n = 2..8 (3pool: n = 3):
+    CFMM_KIND_STABLESWAP_N = 5, /* n-coin StableSwap (Curve), arity n = 2..8 (3pool: n = 3):
                               A n^n sum(y) + D >= A n^n D + D^(n+1) / (n^n prod y), y_j = r_j x_j, D = D(R); at n = 2
                               this is CFMM_KIND_STABLESWAP.  weights [n][stride] = the rates; logrw [2][stride]: slot 0 =
                               A (whitepaper, as kind 4), slot 1 = D.  cfmm_eval_out.hcoef is [n][stride]: the per-slot
                               h_j of the pool's scaled Hessian Hs = C - (C1)(C1)'/(1'C1), C = diag(h^2) - h h'/(1+k)
                               on its k traded slots (hmask), 0 on the others.  Arity 2 is accepted so both kinds can
                               run the same pools; the Python layer sends only n >= 3 here                             */
+    CFMM_KIND_CONCENTRATED = 6 /* concentrated liquidity, a whole Uniswap-v3 tick ladder as one pool: sqrt-price bounds
+                              b_0 < ... < b_T (price = token 1 per token 0), liquidity L_k >= 0 on [b_k, b_{k+1}), the
+                              trading set the Minkowski sum of the intervals' bounded products.  Not in the reference;
+                              arity 2.  weights = the records, AoS, 4 f64 per bound {b_k, L_k, Y_k, X_k} with
+                              Y_k = sum_{j<k} L_j (b_{j+1} - b_j), X_k = sum_{j>=k} L_j (1/b_j - 1/b_{j+1}), L_T = 0;
+                              a pool's T + 1 records are consecutive.  logrw [4][stride]: per pool slot 0 = the current
+                              sqrt price s in [b_0, b_T], slot 1 = c (b_c <= s < b_{c+1}, c <= T - 1), slot 2 = the
+                              index of its first record in `weights`, slot 3 = T (1 <= T <= 2^20); the integers are
+                              exact in f64.  reserves [2][stride] = the real reserves (x, y) at s (not read by the
+                              evaluation).  hcoef is per pool, as for every pair kind: the liquidity of the interval the
+                              trade ends in (at an exact bound, the one above it; 0 past either end) times
+                              sqrt(nu0 nu1 / gamma) / 2.  Smooth between bounds: no theta_bar                        */
 };
 
 enum {
@@ -67,8 +80,8 @@ typedef struct cfmm_bucket {
     const double* reserves;
     const int32_t* tok_idx;
     const double* gamma;
-    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates */
-    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D) */
+    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates; CONCENTRATED records */
+    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D); CONCENTRATED (s, c, first record, T) */
     const double* theta_bar; /* SUM only     */
 } cfmm_bucket;
 
@@ -282,12 +295,14 @@ typedef struct cfmm_csr_pools {
     const int32_t* tok_idx;    /* [nnz]  local_indices, arbitrage.py:6-12                             */
     const double* reserves;    /* [nnz]  arbitrage.py:14-20                                          */
     const double* weights;     /* [nnz]  normalised like cp.geo_mean(p=...), arbitrage.py:65; 0 on constant-sum pools;
-                                         offsets of bounded products; rates of StableSwap pools        */
+                                         offsets of bounded products; rates of StableSwap pools; concentrated
+                                         pools: the sqrt price s at the first slot, c at the second     */
     const double* logrw;       /* [nnz]  log(reserves / weights) (unused on constant-sum pools); StableSwap: A at the
-                                         pool's first slot, D at its second                            */
+                                         pool's first slot, D at its second; concentrated pools: the index of
+                                         the first record at the first slot, T at the second           */
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
-    const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP, else
-                                            weighted geometric mean                                  */
+    const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP |
+                                            CFMM_KIND_CONCENTRATED, else weighted geometric mean     */
 } cfmm_csr_pools;
 
 typedef struct cfmm_batch {
@@ -329,6 +344,12 @@ int cfmm_batch_solve_stableswap(const cfmm_csr_pools* pools, const cfmm_batch* b
  * their registers.  Same arguments, limits and workspace. */
 int cfmm_batch_solve_stableswap_n(const cfmm_csr_pools* pools, const cfmm_batch* batch, const cfmm_batch_params* prm,
                                   void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_CONCENTRATED pools, beside every kind cfmm_batch_solve_stableswap_n
+ * takes (the three entry points above give their problems status 3).  records: the concentrated pools' records (the
+ * AoS layout of CFMM_KIND_CONCENTRATED, device), indexed by the first-record slots of the CSR logrw; CFMM_E_NULL if
+ * NULL.  A fourth kernel instance, so the others keep their registers.  Same limits and workspace. */
+int cfmm_batch_solve_concentrated(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
+                                  const cfmm_batch_params* prm, void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
