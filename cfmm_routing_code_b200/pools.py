@@ -59,21 +59,25 @@ def ladder_state(lad_ptr, lad_rec, pool_ids, prices):
     ptr = np.asarray(lad_ptr, np.int64)
     rec = np.asarray(lad_rec, np.float64).reshape(-1, 4)
     first = ptr[ids]
-    T = ptr[ids + 1] - first - 1
+    return _ladder_state(lambda i, k: rec[i, k], first, ptr[ids + 1] - first - 1, prices)
+
+
+def _ladder_state(col, first, T, prices):
+    """ladder_state on pools given by their first record and T, with col(i, k) = column k of records i"""
     with np.errstate(invalid="ignore"):
-        s = np.minimum(np.maximum(np.sqrt(np.asarray(prices, np.float64).reshape(-1)), rec[first, 0]), rec[first + T, 0])
-    lo, hi = np.zeros(len(ids), np.int64), T - 1                     # the largest c in [lo, hi] with b_c <= s
+        s = np.minimum(np.maximum(np.sqrt(np.asarray(prices, np.float64).reshape(-1)), col(first, 0)), col(first + T, 0))
+    lo, hi = np.zeros(len(first), np.int64), T - 1                   # the largest c in [lo, hi] with b_c <= s
     for _ in range(24):
         act = lo < hi
         if not act.any():
             break
         mid = (lo + hi + 1) // 2
-        up = act & (rec[first + mid, 0] <= s)
+        up = act & (col(first + mid, 0) <= s)
         lo = np.where(up, mid, lo)
         hi = np.where(act & ~up, mid - 1, hi)
     c = lo
-    bc, Lc, Yc = (rec[first + c, k].astype(np.longdouble) for k in (0, 1, 2))
-    bc1, Xc1 = (rec[first + c + 1, k].astype(np.longdouble) for k in (0, 3))
+    bc, Lc, Yc = (col(first + c, k).astype(np.longdouble) for k in (0, 1, 2))
+    bc1, Xc1 = (col(first + c + 1, k).astype(np.longdouble) for k in (0, 3))
     sl = s.astype(np.longdouble)
     y = (Yc + Lc * (sl - bc)).astype(np.float64)
     x = (Xc1 + Lc * ((bc1 - sl) / (sl * bc1))).astype(np.float64)
@@ -93,6 +97,94 @@ def _check_ladder(price, bounds, liquidity, where=""):
         raise ValueError(f"{where}concentrated bounds must be finite, > 0 and strictly increasing")
     if not bool(np.all(np.isfinite(L) & (L >= 0))) or not bool(np.any(L > 0)):
         raise ValueError(f"{where}concentrated liquidity must be finite, >= 0 and not all zero")
+
+
+def new_ladders(ladders):
+    """Records and state of concentrated pools given as (price, bounds, liquidity) triples (already checked), each as
+    HostPools.from_lists makes them: ladder_records of the pool alone (pools of equal T share one call; its rows do not
+    interact) and ladder_state at its price.  Returns (records (sum(T + 1), 4) pool after pool, counts T + 1 (n,) int64,
+    s, c, x, y (n,) f64)."""
+    n = len(ladders)
+    T = np.asarray([len(np.asarray(l[2]).reshape(-1)) for l in ladders], np.int64)
+    recs = [None] * n
+    for t in np.unique(T).tolist():
+        sel = np.nonzero(T == t)[0].tolist()
+        B = np.stack([np.asarray(ladders[k][1], np.float64).reshape(-1) for k in sel])
+        L = np.stack([np.asarray(ladders[k][2], np.float64).reshape(-1) for k in sel])
+        for k, r in zip(sel, ladder_records(B, L)):
+            recs[k] = r
+    cnt = T + 1
+    rec = np.concatenate(recs) if n else np.zeros((0, 4))
+    ptr = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+    s, c, x, y = ladder_state(ptr, rec, np.arange(n), [float(l[0]) for l in ladders])
+    return rec, cnt, s, c, x, y
+
+
+class LadderSlab:
+    """The host records of a store's concentrated pools, replaceable pool by pool (PoolStore.update_pools(ladders=)).
+    Pool i's T[i] + 1 records start at first[i] of the concatenation [base | own] (T[i] = -1: not a ladder): `base` is
+    a HostPools' lad_rec, borrowed and never written, `own` an append-only slab of the ladders that replaced others.  A
+    replacement appends its records and leaves the ones it supersedes dead; once the dead records outnumber the live
+    ones, the live ones are compacted into a new slab in pool order and the base is let go.  So one replacement costs
+    O(its records) plus O(m) integer work, amortised, not a copy of every record."""
+
+    def __init__(self, lad_ptr, lad_rec):
+        ptr = np.asarray(lad_ptr, np.int64)
+        self.base = np.asarray(lad_rec, np.float64).reshape(-1, 4)
+        self.first = ptr[:-1].copy()
+        self.T = np.diff(ptr) - 1
+        self.own = np.zeros((0, 4))
+        self.n_own = 0
+        self.live, self.dead = int(ptr[-1]), 0
+
+    def col(self, i, k):
+        """column k of records i (indices into [base | own])"""
+        nb = len(self.base)
+        if self.n_own == 0:
+            return self.base[i, k]
+        if nb == 0:
+            return self.own[i, k]
+        inb = i < nb
+        return np.where(inb, self.base[np.where(inb, i, 0), k], self.own[np.where(inb, 0, i - nb), k])
+
+    def records(self, pool: int) -> np.ndarray:
+        """(T + 1, 4) records of one pool"""
+        i = self.first[pool] + np.arange(self.T[pool] + 1)
+        return np.stack([self.col(i, k) for k in range(4)], 1)
+
+    def state(self, ids, prices):
+        """ladder_state of pools ids at new prices, from these records"""
+        ids = np.asarray(ids, np.int64)
+        return _ladder_state(self.col, self.first[ids], self.T[ids], prices)
+
+    def replace(self, ids, rec, cnt):
+        """pools ids (distinct, concentrated) take new records rec, cnt[k] of them for ids[k], pool after pool"""
+        ids = np.asarray(ids, np.int64)
+        old = int((self.T[ids] + 1).sum())
+        need = len(rec)
+        if self.n_own + need > len(self.own):                         # grow geometrically: appends stay amortised O(1)
+            grown = np.empty((max(2 * len(self.own), self.n_own + need), 4))
+            grown[:self.n_own] = self.own[:self.n_own]
+            self.own = grown
+        self.own[self.n_own:self.n_own + need] = rec
+        self.first[ids] = len(self.base) + self.n_own + np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
+        self.T[ids] = np.asarray(cnt, np.int64) - 1
+        self.n_own += need
+        self.live += need - old
+        self.dead += old
+        if self.dead > self.live:
+            self._compact()
+
+    def _compact(self):
+        lad = np.nonzero(self.T >= 0)[0]
+        cnt = self.T[lad] + 1
+        start = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
+        i = np.repeat(self.first[lad] - start, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
+        self.own = np.stack([self.col(i, k) for k in range(4)], 1)
+        self.base = np.zeros((0, 4))
+        self.n_own = len(self.own)
+        self.first[lad] = start
+        self.live, self.dead = self.n_own, 0
 
 
 def stableswap_invariant(reserves, rates, amp) -> np.ndarray:
@@ -402,25 +494,45 @@ class PoolUpdate:
     reserves: Optional[np.ndarray]   # f64 [nnz] new reserves at `slots`, or None
     gamma: Optional[np.ndarray]      # f64 [n] new fees, or None
     prices: Optional[np.ndarray] = None   # f64 [n] new prices of concentrated pools, or None
+    ladders: Optional[list] = None        # [n] new (price, bounds f64, liquidity f64) of concentrated pools, or None
+    amp: Optional[np.ndarray] = None      # f64 [n] new amplifications A of StableSwap pools, or None
+    rates: Optional[np.ndarray] = None    # f64 [nnz] new rates of StableSwap pools at `slots`, or None
+
+
+def _pool_rows(vals, n, ar, what):
+    """per-pool vectors of the pools' arities (a list, or an (n, k) array when all have arity k), flattened in order"""
+    if isinstance(vals, np.ndarray) and vals.ndim == 2:
+        if len(vals) != n or (n and bool(np.any(ar != vals.shape[1]))):
+            raise ValueError(f"{what}: one row per pool, of the pool's arity")
+        return np.ascontiguousarray(vals, np.float64).reshape(-1)
+    if len(vals) != n:
+        raise ValueError(f"{what}: one vector per pool")
+    rows = [np.asarray(r, np.float64).reshape(-1) for r in vals]
+    if any(len(r) != a for r, a in zip(rows, ar.tolist())):
+        raise ValueError(f"{what}: a vector's length differs from its pool's arity")
+    return np.concatenate(rows) if rows else np.zeros(0)
 
 
 def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarray, pool_ids, reserves=None,
-                      fees=None, prices=None) -> PoolUpdate:
+                      fees=None, prices=None, ladders=None, amp=None, rates=None) -> PoolUpdate:
     """Host checks of PoolStore.update_pools, on the problem's CSR arrays (pool_ptr, kind, weights as in HostPools).
     pool_ids: global pool indices, distinct and in range; reserves[k]: the new reserve vector of pool pool_ids[k] with the
     pool's arity (a row of the reference's `reserves` literal; an (n, k) array when all pools have arity k); fees[k]: its
     new gamma.  The values must pass the rules of HostPools.validate (bounded_product pools with their own offsets).
     prices[k]: the new price (token 1 per token 0) of pool pool_ids[k], which must then be concentrated; a concentrated pool
-    takes no reserves (they are derived from its price).
-    Raises ValueError; returns the update with the reserves flattened into the pools' CSR slot order."""
+    takes no reserves (they are derived from its price).  ladders[k]: the new (price, bounds, liquidity) of concentrated
+    pool pool_ids[k], the triple of HostPools.from_lists' weights[i] (T may differ from the pool's old T; the rules of
+    from_lists); not together with prices=.  amp[k]: the new whitepaper A of StableSwap pool pool_ids[k], rates[k]: its new
+    rate vector (the pool's arity; an (n, k) array as for reserves), under the rules of from_lists.
+    Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order."""
     m = len(pool_ptr) - 1
     ids = np.asarray(pool_ids)
     if ids.ndim != 1 or (ids.size and not np.issubdtype(ids.dtype, np.integer)):
         raise ValueError("pool_ids must be a 1-d sequence of integer pool indices")
     ids = ids.astype(np.int64)
     n = len(ids)
-    if reserves is None and fees is None and prices is None:
-        raise ValueError("nothing to update: give reserves, fees, prices or several")
+    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates)):
+        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates or several")
     if n and (ids.min() < 0 or ids.max() >= m):
         raise ValueError(f"pool id out of range [0, {m})")
     conc = np.asarray(kind)[ids] == KIND_CONCENTRATED_HOST
@@ -448,17 +560,7 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
         slots = np.repeat(pool_ptr[ids] - first[:-1], ar) + np.arange(first[-1], dtype=np.int64)
     R = None
     if reserves is not None:
-        if isinstance(reserves, np.ndarray) and reserves.ndim == 2:
-            if len(reserves) != n or (n and bool(np.any(ar != reserves.shape[1]))):
-                raise ValueError("reserves: one row per pool, of the pool's arity")
-            R = np.ascontiguousarray(reserves, np.float64).reshape(-1)
-        else:
-            if len(reserves) != n:
-                raise ValueError("reserves: one vector per pool")
-            rows = [np.asarray(r, np.float64).reshape(-1) for r in reserves]
-            if any(len(r) != a for r, a in zip(rows, ar.tolist())):
-                raise ValueError("reserves: a vector's length differs from its pool's arity")
-            R = np.concatenate(rows) if rows else np.zeros(0)
+        R = _pool_rows(reserves, n, ar, "reserves")
         bounded = np.repeat(np.asarray(kind)[ids] == KIND_BOUNDED_HOST, ar)
         if bounded.any():
             virt = R + np.where(bounded, weights[slots], 0.0)
@@ -474,7 +576,37 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             raise ValueError("fees: one per pool")
         if not bool(np.all((g > 0) & (g <= 1))):
             raise ValueError("fees (gamma) must lie in (0, 1]")
-    return PoolUpdate(ids, first, slots, R, g, pr)
+    lad = None
+    if ladders is not None:
+        if prices is not None:
+            raise ValueError("ladders= and prices= cannot be combined (a ladder carries its price)")
+        if len(ladders) != n:
+            raise ValueError("ladders: one (price, bounds, liquidity) per pool")
+        if not bool(np.all(conc)):
+            raise ValueError("ladders= applies to concentrated pools only")
+        lad = []
+        for k, t in enumerate(ladders):
+            if t is None or len(t) != 3:
+                raise ValueError(f"ladders[{k}]: concentrated needs (price, bounds, liquidity)")
+            _check_ladder(t[0], t[1], t[2], f"ladders[{k}]: ")
+            lad.append((float(np.asarray(t[0], np.float64).reshape(-1)[0]), np.asarray(t[1], np.float64).reshape(-1),
+                        np.asarray(t[2], np.float64).reshape(-1)))
+    A = W = None
+    if amp is not None or rates is not None:
+        if not bool(np.all(np.asarray(kind)[ids] == KIND_STABLESWAP_HOST)):
+            raise ValueError("amp= and rates= apply to StableSwap pools only")
+        if amp is not None:
+            A = np.ascontiguousarray(amp, np.float64).reshape(-1)
+            if len(A) != n:
+                raise ValueError("amp: one per pool")
+        if rates is not None:
+            W = _pool_rows(rates, n, ar, "rates")
+        for k in np.unique(ar).tolist():         # the rules of from_lists per coin count (ones stand in for what is kept)
+            sel = np.nonzero(ar == k)[0]
+            _check_stableswap(np.ones(len(sel)) if A is None else A[sel],
+                              np.ones((len(sel), k)) if W is None else W[first[sel][:, None] + np.arange(k)],
+                              np.ones((len(sel), k)))
+    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W)
 
 
 class BucketSpec:
@@ -623,6 +755,8 @@ class DeviceBucket:
             loc = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
             gather = np.repeat(first - loc, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
             self.weights = torch.as_tensor(np.ascontiguousarray(np.asarray(hp.lad_rec, np.float64)[gather]).reshape(-1), **f64)
+            self.n_rec = int(cnt.sum())
+            self._rec_buf, self._rec_spare = self.weights, None      # splice_ladders writes the spare and swaps
             sc = np.asarray(hp.lad_sc, np.float64)[sel]
             P = np.stack([sc[:, 0], sc[:, 1], loc.astype(np.float64), (cnt - 1).astype(np.float64)])
             self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
@@ -646,10 +780,12 @@ class DeviceBucket:
         return self.spec.off
 
     def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
-                     W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None, sc: Optional[np.ndarray] = None):
+                     W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None, sc: Optional[np.ndarray] = None,
+                     rates: Optional[np.ndarray] = None, AD: Optional[np.ndarray] = None):
         """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
         Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__;
-        StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,);
+        StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,), or, when
+        their A or rates change, the new rates (arity, n) in the weights rows and AD = (A, D) (2, n) in logrw rows 0-1;
         concentrated pools get their new (s, c) from sc (2, n), with R their derived reserves (ladder_state)."""
         f64 = dict(dtype=torch.float64, device=self._device)
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
@@ -658,11 +794,48 @@ class DeviceBucket:
         if R is not None:
             self.reserves[:, li] = torch.as_tensor(R, **f64)
             if self.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N):
-                self.logrw[1, li] = torch.as_tensor(stableswap_invariant_any(R.T, W.T, amp), **f64)
+                if AD is None:
+                    self.logrw[1, li] = torch.as_tensor(stableswap_invariant_any(R.T, W.T, amp), **f64)
             elif self.kind == _lib.KIND_GEOMEAN:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
+        if rates is not None:
+            self.weights[:, li] = torch.as_tensor(rates, **f64)
+        if AD is not None:
+            self.logrw[:2, li] = torch.as_tensor(AD, **f64)
         if gamma is not None:
             self.gamma[li] = torch.as_tensor(gamma, **f64)
+
+    def splice_ladders(self, lib, loc: np.ndarray, rec: np.ndarray, cnt: np.ndarray, state: np.ndarray, n_total: int,
+                       stream):
+        """New ladders of the concentrated pools at the bucket-local positions `loc` (ascending): their records rec
+        (sum(cnt), 4), pool after pool, cnt[k] = T + 1 of pool loc[k], state (n, 4) = (s, c, x, y).  cfmm_ladder_splice
+        writes every pool's records into the spare buffer in bucket order (n_total of them), then the two buffers swap, so
+        c_bucket.weights moves (a CUDA graph captured over this bucket must be captured again).  Synchronous."""
+        dev = self._device
+        if self._rec_spare is None or self._rec_spare.numel() < 4 * n_total:
+            self._rec_spare = None
+            self._rec_spare = torch.empty(4 * (n_total + n_total // 8), dtype=torch.float64, device=dev)
+        f64 = dict(dtype=torch.float64, device=dev)
+        pos = torch.as_tensor(np.asarray(loc, np.int64), device=dev)
+        nrec = torch.as_tensor(np.asarray(cnt, np.int64), device=dev)
+        recd = torch.as_tensor(np.ascontiguousarray(rec, np.float64), **f64)
+        std = torch.as_tensor(np.ascontiguousarray(state, np.float64), **f64)
+        nb = int(lib.cfmm_ladder_splice_work_bytes(self.m, len(loc)))
+        if nb < 0:
+            _lib.check(nb, "cfmm_ladder_splice_work_bytes")
+        work = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
+        status = (C.c_int64 * 2)()
+        _lib.check(lib.cfmm_ladder_splice(C.byref(self.c_bucket), len(loc), pos.data_ptr(), nrec.data_ptr(),
+                                          recd.data_ptr(), len(rec), std.data_ptr(), self._rec_spare.data_ptr(),
+                                          self._rec_spare.numel() // 4, status, work.data_ptr(), nb, stream),
+                   "cfmm_ladder_splice")
+        if status[0] != 0 or status[1] != n_total:
+            raise _lib.CfmmError(f"cfmm_ladder_splice rejected the update ({status[0]} invalid entries, {status[1]} records "
+                                 f"for {n_total} expected)")
+        self._rec_buf, self._rec_spare = self._rec_spare, self._rec_buf
+        self.weights = self._rec_buf[:4 * n_total]
+        self.n_rec = n_total
+        self.c_bucket.weights = self.weights.data_ptr()
 
     def bytes_resident(self) -> int:
         n = 0
@@ -1103,9 +1276,13 @@ class PoolStore:
         self.m_total = hp.m
         self.pool_ptr = hp.pool_ptr
         self._tok_idx_host = hp.tok_idx
+        # borrowed from hp and never written: update_pools(amp=, rates=) copies weights and amp first, and ladders live in
+        # a LadderSlab over hp's records (made at the first update that needs them)
         self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets / rates
-        self._amp_host = hp.amp                                          # StableSwap amplification (structure too)
-        self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records (structure)
+        self._amp_host = hp.amp                                          # StableSwap amplification
+        self._own_stable = False                                         # weights / amp are this store's copies
+        self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records
+        self._lad = None                                                 # LadderSlab
         self._where = None                                               # pool -> (bucket, position): update_pools
         self.rank, self.world = rank, world
         self.buckets = []
@@ -1281,28 +1458,44 @@ class PoolStore:
             self._where = (bi, loc)
         return self._where
 
-    def update_pools(self, pool_ids, reserves=None, fees=None, prices=None):
-        """Set new reserves and / or fees of some pools in place: the store then equals, bit for bit, a PoolStore built
-        from the updated host data, without re-uploading the pools or rebuilding the blocked layout (which depends on the
-        token ids only).  pool_ids: global pool indices (the order of the problem's local_indices); reserves[k]: the new
-        reserve vector of pool pool_ids[k], with the pool's arity (an (n, 2) array for pairs); fees[k]: its new gamma in
-        (0, 1].  At least one of reserves / fees.  Kinds, tokens, weights, bounded_product offsets and StableSwap
-        amplifications and rates cannot change (they are structure: build a new store, e.g. for a ramp of A); a StableSwap
-        pool's invariant D is recomputed from its new reserves, as HostPools does.  Concentrated pools take prices=
-        (prices[k]: the new price of pool pool_ids[k], token 1 per token 0) instead of reserves=, which raises for them:
-        their (s, c) and real reserves are recomputed with ladder_state, the function HostPools uses, and their records
-        (bounds and liquidity, i.e. mints and burns) are structure.
+    def _ladders(self) -> LadderSlab:
+        if self._lad is None:
+            self._lad = LadderSlab(*self._lad_host)
+        return self._lad
 
-        All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.validate) raise
-        ValueError before anything is written, and so does an entry the device check of the blocked bucket rejects.
-        Pools held by other ranks of a sharded store are skipped: give every rank the same full update.  The caller's
-        HostPools is not modified (the store reads no host reserve or fee after construction).  Synchronous.  Returns
-        the number of blocked tiles whose fee record was rebuilt.
+    def update_pools(self, pool_ids, reserves=None, fees=None, prices=None, ladders=None, amp=None, rates=None):
+        """Set new reserves, fees, prices, ladders, amplifications and / or rates of some pools in place: the store then
+        equals, bit for bit, a PoolStore built from a HostPools of the updated literals, without re-uploading the pools or
+        rebuilding the blocked layout (which depends on the token ids only).  pool_ids: global pool indices (the order of
+        the problem's local_indices); reserves[k]: the new reserve vector of pool pool_ids[k], with the pool's arity (an
+        (n, 2) array for pairs); fees[k]: its new gamma in (0, 1].  At least one keyword.  Kinds, tokens, coin counts,
+        weighted pools' weights and bounded_product offsets cannot change (they are structure: build a new store).
+        A StableSwap pool's invariant D is recomputed from its new reserves, as HostPools does.  amp[k] / rates[k] (StableSwap
+        pools only): its new whitepaper A / rate vector (a ramp of A, a moved rate oracle); D is then recomputed with
+        stableswap_invariant_any from the pool's reserves after the call (the new ones if reserves= is given, else its
+        current ones, read back from the device), and later reserves= updates use the new A and rates.
+        Concentrated pools take prices= (prices[k]: the new price of pool pool_ids[k], token 1 per token 0) instead of
+        reserves=, which raises for them: their (s, c) and real reserves are recomputed with ladder_state, the function
+        HostPools uses.  ladders[k] = (price, bounds, liquidity) (concentrated pools only, not with prices=): the pool's
+        whole new ladder, the triple of HostPools.from_lists (instances.v3_ladder of its on-chain state after a Mint or
+        Burn); T may change (1 .. LADDER_T_MAX).  Its records are made by ladder_records, as from_lists does, and
+        cfmm_ladder_splice rewrites the bucket's records into a second device buffer, which the bucket then uses: a
+        ladders= update moves the bucket's records pointer, so a CUDA graph captured over this store must be captured
+        again.  The device keeps two record buffers of the concentrated bucket from the first ladders= update on.
+
+        All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.from_lists and
+        validate) raise ValueError before anything is written on the device or in the store's host state, and so does an
+        entry the device check of the blocked bucket rejects.  Pools held by other ranks of a sharded store are skipped:
+        give every rank the same full update.  The caller's HostPools is not modified: the store reads no host reserve or
+        fee after construction, and keeps its own copies of the rates, amplifications (copied whole at the first amp= /
+        rates= update) and ladder records (a LadderSlab: appends, not copies of every record).  Synchronous.  Returns the
+        number of blocked tiles whose fee record was rebuilt.
 
         A new block of the same market is then re-solved warm from the previous prices:
             store.update_pools(ids, reserves=new_R, fees=new_gamma)
             res = solve_pools(hp, utility, store=store, nu0=res.nu)"""
-        u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees, prices)
+        u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees, prices,
+                              ladders, amp, rates)
         bi, loc = self._pool_map()
         owner = bi[u.ids]
         plan = []
@@ -1310,24 +1503,53 @@ class PoolStore:
             e = np.nonzero(owner == k)[0]
             if len(e) == 0:
                 continue
+            if u.ladders is not None:                # concentrated pools only (checked): the splice takes them in order
+                e = e[np.argsort(loc[u.ids[e]], kind="stable")]
             rs = u.ptr[e][None, :] + np.arange(b.arity)[:, None]          # (arity, n) indices into the update's slots
+            ids = u.ids[e]
             R = None if u.reserves is None else u.reserves[rs]
             g = None if u.gamma is None else u.gamma[e]
-            sc = None
+            sc = lad = rt = AD = None
             if u.prices is not None:                 # concentrated pools only (checked): state and reserves at the price
-                s, c, x, y = ladder_state(self._lad_host[0], self._lad_host[1], u.ids[e], u.prices[e])
+                s, c, x, y = (self._lad.state(ids, u.prices[e]) if self._lad is not None else
+                              ladder_state(self._lad_host[0], self._lad_host[1], ids, u.prices[e]))
                 sc, R = np.stack([s, c]), np.stack([x, y])
-            plan.append((b, loc[u.ids[e]], R, g, rs, u.ids[e], sc))
+            if u.ladders is not None:                # new records and state, as HostPools.from_lists makes them
+                rec, cnt, s, c, x, y = new_ladders([u.ladders[j] for j in e.tolist()])
+                n_total = b.n_rec + int(cnt.sum()) - int((self._ladders().T[ids] + 1).sum())
+                lad = (rec, cnt, np.stack([s, c, x, y], 1), n_total)
+            if u.amp is not None or u.rates is not None:   # StableSwap pools only (checked): D of the reserves after the call
+                A = u.amp[e] if u.amp is not None else self._amp_host[ids]
+                rt = u.rates[rs] if u.rates is not None else self._weights_host[u.slots[rs]]
+                Rd = R if R is not None else b.reserves[:, torch.as_tensor(loc[ids], device=self.device)].cpu().numpy()
+                D = stableswap_invariant_any(Rd.T, rt.T, A)
+                if not bool(np.all(np.isfinite(D) & (D > 0))):
+                    raise ValueError("stableswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
+                AD = np.stack([A, D])
+            plan.append((b, loc[ids], R, g, rs, ids, sc, lad, rt, AD))
         # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
         rebuilt = 0
-        for b, l, R, g, _, _, _ in plan:
+        for b, l, R, g, *_ in plan:
             if getattr(b, "blocked", False):
                 rebuilt += b.write_update(self.lib, l, R, g, self._stream())
-        for b, l, R, g, rs, ids, sc in plan:
-            if not getattr(b, "blocked", False):
-                W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None) else None
-                amp = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) else None
-                b.write_update(l, R, g, W, amp, sc)
+        for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:
+            if getattr(b, "blocked", False):
+                continue
+            if lad is not None:
+                b.splice_ladders(self.lib, l, lad[0], lad[1], lad[2], lad[3], self._stream())
+            W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None and AD is None) else None
+            amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) else None
+            b.write_update(l, R, g, W, amp_, sc, None if u.rates is None else rt, AD)
+        # the store's host state, once the device holds the update
+        for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:
+            if lad is not None:
+                self._ladders().replace(ids, lad[0], lad[1])
+            if AD is not None:
+                if not self._own_stable:
+                    self._weights_host, self._amp_host = self._weights_host.copy(), self._amp_host.copy()
+                    self._own_stable = True
+                self._amp_host[ids] = AD[0]
+                self._weights_host[u.slots[rs]] = rt
         torch.cuda.synchronize(self.device)
         return rebuilt
 

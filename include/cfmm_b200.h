@@ -204,6 +204,28 @@ int64_t cfmm_blocked_update_work_bytes(const cfmm_blocked_pairs* b);
 int cfmm_blocked_update(const cfmm_blocked_pairs* b, int64_t n_upd, const uint32_t* at, const double* reserves,
                         const double* gamma, int32_t* status_host, void* work, int64_t work_bytes, void* stream);
 
+/*
+ * New tick ladders for n_chg pools of a CFMM_KIND_CONCENTRATED bucket (mints and burns; T may change), spliced into a
+ * second record buffer.  pos [n_chg] int64: the changed BUCKET-LOCAL positions, strictly increasing, < b->n_pools;
+ * n_rec [n_chg] int64: their new record counts T + 1 (2 .. 2^20 + 1); records [n_records][4] f64: their new records
+ * (the AoS layout of CFMM_KIND_CONCENTRATED), pool after pool in `pos` order; state [n_chg][4] f64: their new
+ * (s, c, x, y).  Every pool's records, old (from b->weights) or new, are copied into out_records [out_capacity][4] in
+ * bucket order, each pool's first record being the exclusive scan of the record counts; logrw rows 2-3 (first record,
+ * T) of every pool and rows 0-1 (s, c) and the reserves of the changed pools are written in place.  b->weights is only
+ * read: the caller points the bucket at out_records afterwards (and keeps the old buffer for the next splice), so a
+ * CUDA graph captured over the bucket must be captured again.  out_records must not overlap b->weights; b->weights,
+ * records and out_records must be 16-byte aligned (CFMM_E_SIZE otherwise).  n_chg = 0 copies the records as they are.
+ * All or nothing: if a position is out of range, repeated or out of order, a count out of range, the counts do not sum
+ * to n_records or the new total exceeds out_capacity, nothing is written (bucket and out_records).
+ * status_host [2] int64 (host, out): [0] invalid entries (nothing was written if > 0), [1] the bucket's new total of
+ * records.  work: cfmm_ladder_splice_work_bytes(b->n_pools, n_chg) bytes of device memory (no initialisation needed).
+ * CFMM_E_KIND unless kind CONCENTRATED, arity 2.  SYNCHRONOUS on `stream`, like cfmm_blocked_update.
+ */
+int64_t cfmm_ladder_splice_work_bytes(int64_t n_pools, int64_t n_chg);
+int cfmm_ladder_splice(const cfmm_bucket* b, int64_t n_chg, const int64_t* pos, const int64_t* n_rec, const double* records,
+                       int64_t n_records, const double* state, double* out_records, int64_t out_capacity,
+                       int64_t* status_host, void* work, int64_t work_bytes, void* stream);
+
 /* Same contract as cfmm_arb_eval for a blocked constant-product bucket: psi/arb ACCUMULATE (one red.add per row
  * of <= 32 entries, ~0.35 per pool, instead of 2 per pool).  Per-pool outputs (delta/lambda [2][n_tiles*P], hcoef
  * [n_tiles*P]) are in BLOCKED order.  If zero_next != NULL the launch also clears zero_next[0..n_zero): callers that
