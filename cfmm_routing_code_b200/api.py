@@ -108,7 +108,10 @@ def solve(local_indices, reserves, fees, kinds, weights=None, utility=None, n_to
     'bounded_product' (weights[i] = virtual-reserve offsets) and 'stableswap' (weights[i] = (A, r_0, ..., r_{n-1}), a
     Curve pool of 2..8 coins with the whitepaper A = A() / n^(n-1); see HostPools.from_lists).  And 'concentrated':
     weights[i] = (price, bounds, liquidity), a whole Uniswap-v3 tick ladder as one pool, with reserves[i] = None (see
-    HostPools.from_lists and instances.v3_ladder)."""
+    HostPools.from_lists and instances.v3_ladder).  And 'cryptoswap': weights[i] = (A, gamma, p_0, p_1), a two-coin Curve v2
+    (twocrypto-ng) pool with the whitepaper A, the curve's gamma and the price scales (see HostPools.from_lists and
+    instances.twocrypto_pool).  Problems with StableSwap, concentrated or cryptoswap pools run solver.py or the per-thread
+    solver, never the native blocked and persistent solvers."""
     if utility is None:
         raise ValueError("utility is required: Arbitrage(c) | Liquidate(target, assets) | Swap(i, o, t)")
     if n_tokens is None:

@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .pools import HostPools, KIND_CONCENTRATED_HOST, KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
+from .pools import HostPools, KIND_CONCENTRATED_HOST, KIND_CRYPTOSWAP_HOST, KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
 from .solver import default_nu0
 
 NTOK_MAX = 64      # cfmm_small::NTOK_MAX
@@ -68,6 +68,17 @@ class CsrStore:
             self.logrw[first] = torch.as_tensor(lp[cl].astype(np.float64), device=dev)
             self.logrw[first + 1] = torch.as_tensor((lp[cl + 1] - lp[cl] - 1).astype(np.float64), device=dev)
             self.records = torch.as_tensor(np.ascontiguousarray(hp.lad_rec, np.float64).reshape(-1), device=dev)
+        cs = np.nonzero(np.asarray(hp.kind) == KIND_CRYPTOSWAP_HOST)[0]
+        self.has_crypto = bool(len(cs))              # -> cfmm_batch_solve_cryptoswap (a fifth instance)
+        if len(cs):                                  # cryptoswap pools: p_j / D in the w slots, (A, G) in logrw
+            first = np.asarray(hp.pool_ptr, np.int64)[cs]
+            Dv = np.asarray(hp.inv, np.float64)[cs]
+            W = np.asarray(hp.weights, np.float64)
+            fd = torch.as_tensor(first, device=dev)
+            self.w[fd] = torch.as_tensor(W[first] / Dv, device=dev)
+            self.w[fd + 1] = torch.as_tensor(W[first + 1] / Dv, device=dev)
+            self.logrw[fd] = torch.as_tensor(np.asarray(hp.amp, np.float64)[cs], device=dev)
+            self.logrw[fd + 1] = torch.as_tensor(np.asarray(hp.cgam, np.float64)[cs], device=dev)
         self.gamma = torch.as_tensor(np.ascontiguousarray(hp.gamma, np.float64), device=dev)
         self.kind = torch.as_tensor(np.ascontiguousarray(hp.kind, np.uint8), device=dev)
         self.c_pools = _lib.CsrPools(self.n_tokens, self.m, self.nnz, self.pool_ptr.data_ptr(), self.tok.data_ptr(),
@@ -120,6 +131,12 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if store.has_crypto:
+        _lib.check(store.lib.cfmm_batch_solve_cryptoswap(C.byref(store.c_pools),
+                                                         store.records.data_ptr() if store.records is not None else None,
+                                                         C.byref(batch), C.byref(prm), work.data_ptr(), st),
+                   "cfmm_batch_solve_cryptoswap")
+        return psi, stats, delta, lam
     if store.has_ladder:
         _lib.check(store.lib.cfmm_batch_solve_concentrated(C.byref(store.c_pools), store.records.data_ptr(),
                                                            C.byref(batch), C.byref(prm), work.data_ptr(), st),
@@ -209,7 +226,8 @@ def pack_problems(problems: Sequence):
                        cat("weights", np.float64), cat("gamma", np.float64), cat("kind", np.uint8),
                        cat("amp", np.float64), cat("inv", np.float64), np.concatenate(lptr),
                        np.concatenate([np.asarray(hp.lad_rec, np.float64).reshape(-1, 4) for hp, _ in problems]),
-                       np.concatenate([np.asarray(hp.lad_sc, np.float64).reshape(-1, 2) for hp, _ in problems]))
+                       np.concatenate([np.asarray(hp.lad_sc, np.float64).reshape(-1, 2) for hp, _ in problems]),
+                       cat("cgam", np.float64))
     return merged, ranges, c, a, fl, nu, nnz_max
 
 

@@ -206,6 +206,40 @@ k_eval_stable(long long m, long long ld, int n_tokens, const double* __restrict_
     block_accumulate(acc, arb);
 }
 
+// two-coin cryptoswap (Curve v2): cfmm_small::cryptoswap_pair (a safeguarded Newton solve per trading pool around an
+// inner one for the curve point, compute-bound), one thread per pool.  scales [2][ld] = the price scales p (the bucket's
+// weights), AGD [3][ld] = (A, G, D) (the bucket's logrw); the kernel passes c = p / D.
+template <typename Scatter, bool TRADES, bool HESS>
+__global__ void __launch_bounds__(kThreads)
+k_eval_crypto(long long m, long long ld, int n_tokens, const double* __restrict__ R, const int* __restrict__ idx,
+              const double* __restrict__ gamma, const double* __restrict__ scales, const double* __restrict__ AGD,
+              const double* __restrict__ nu, double* psi, double* arb, double* delta, double* lambda, double* hcoef) {
+    extern __shared__ double smem[];
+    Scatter sc{psi};
+    sc.init(smem, n_tokens);
+    double acc = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        const int i0 = idx[i], i1 = idx[ld + i];
+        const double n0 = __ldg(nu + i0), n1 = __ldg(nu + i1);
+        const double Dv = AGD[2 * ld + i];
+        double D[2], L[2], h;
+        cfmm_small::cryptoswap_pair(R[i], R[ld + i], scales[i] / Dv, scales[ld + i] / Dv, AGD[i], AGD[ld + i], gamma[i],
+                                    n0, n1, D, L, h);
+        const double y0 = L[0] - D[0], y1 = L[1] - D[1];
+        if (TRADES) {
+            delta[i] = D[0]; delta[ld + i] = D[1];
+            lambda[i] = L[0]; lambda[ld + i] = L[1];
+        }
+        if (HESS) hcoef[i] = h;
+        if (y0 != 0.0) sc.add(i0, y0);
+        if (y1 != 0.0) sc.add(i1, y1);
+        acc += n0 * y0 + n1 * y1;
+    }
+    sc.flush(smem, n_tokens);
+    block_accumulate(acc, arb);
+}
+
 // concentrated liquidity (a whole tick ladder per pool): cfmm_small::ladder_pair, one thread per pool.  rec = the AoS
 // records (the bucket's weights), P [4][ld] = (s, c, first record, T) (the bucket's logrw).  The reserves are not read:
 // the flows come from the records.  A trade that stays in the current interval reads records c and c + 1; one that
@@ -791,6 +825,28 @@ int launch_stable(const cfmm_bucket* b, int n_tokens, const double* nu, double* 
     return check_launch();
 }
 
+// cryptoswap buckets: the LDG path only, as for StableSwap
+template <bool TRADES, bool HESS>
+int launch_crypto(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                  const cfmm_eval_out* out, cudaStream_t st) {
+    const long long m = b->n_pools;
+    double* delta = out ? out->delta : nullptr;
+    double* lambda = out ? out->lambda : nullptr;
+    double* hcoef = out ? out->hcoef : nullptr;
+    if (use_shared(n_tokens, m)) {
+        const size_t sm = (size_t)n_tokens * sizeof(double);
+        auto kern = k_eval_crypto<SharedScatter, TRADES, HESS>;
+        allow_smem(kern, sm);
+        kern<<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights,
+                                                    b->logrw, nu, psi, arb, delta, lambda, hcoef);
+    } else {
+        k_eval_crypto<GlobalScatter, TRADES, HESS><<<grid_for(m, 8), kThreads, 0, st>>>(
+            m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights, b->logrw, nu, psi, arb, delta, lambda,
+            hcoef);
+    }
+    return check_launch();
+}
+
 // n-coin StableSwap buckets: the LDG path only, as for two coins
 template <int K, bool TRADES, bool HESS>
 int launch_stable_n(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
@@ -853,6 +909,8 @@ int launch_kind(const cfmm_bucket* b, int n_tokens, const double* nu, double eps
         return launch_ladder<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
     else if constexpr (KIND == CFMM_KIND_STABLESWAP)
         return launch_stable<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
+    else if constexpr (KIND == CFMM_KIND_CRYPTOSWAP)
+        return launch_crypto<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
     else
         return launch_pair<KIND, TRADES, HESS>(b, n_tokens, nu, eps, psi, arb, out, st);
 }
@@ -931,6 +989,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 2) return CFMM_E_KIND;
             if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // records; (s, c, first, T)
             break;
+        case CFMM_KIND_CRYPTOSWAP:
+            if (b->arity != 2) return CFMM_E_KIND;
+            if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // price scales; (A, G, D)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -962,6 +1024,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_STABLESWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_CONCENTRATED:
             return dispatch_pair<CFMM_KIND_CONCENTRATED>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_CRYPTOSWAP:
+            return dispatch_pair<CFMM_KIND_CRYPTOSWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP_N:
             switch (b->arity) {
                 case 2: return dispatch_stable_n<2>(b, n_tokens, nu, psi, arb, out, st);

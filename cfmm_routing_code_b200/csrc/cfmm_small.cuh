@@ -36,11 +36,12 @@ struct Pools {                       // CSR problem data (device pointers in the
     const int32_t* tok;              // [nnz]   token of every slot            arbitrage.py:6-12
     const double* R;                 // [nnz]   reserves                       arbitrage.py:14-20
     const double* w;                 // [nnz]   normalised weights | 0 on constant-sum pools | virtual offsets (kind 3) |
-                                     //         rates (kind 4)
-    const double* logrw;             // [nnz]   log(R/w) | kind 4: A at the pool's first slot, its invariant D at the second
+                                     //         rates (kind 4) | p_j / D (kind 8)
+    const double* logrw;             // [nnz]   log(R/w) | kind 4: A at the pool's first slot, its invariant D at the second |
+                                     //         kind 8: A, then the curve gamma G
     const double* gamma;             // [m]     fees                           arbitrage.py:22-28
     const uint8_t* kind;             // [m]     1 = constant sum; 3 = bounded-liquidity product; 4 = StableSwap (2 coins;
-                                     //         2..KMAX in the STABLE_N instance);
+                                     //         2..KMAX in the STABLE_N instance); 8 = two-coin cryptoswap (CRYPTO instance);
                                      //         0 or 2 = weighted geometric mean
                                      //         (constant product = equal weights)
 };
@@ -270,6 +271,123 @@ CFMM_HD inline void stableswap_pair(double R0, double R1, double r0, double r1, 
     double d0, l1, d1, l0;
     hc = stableswap_dir(R0, R1, r0, r1, u0, u1, mu0, mu1, n0, A, Dinv, gam, d0, l1)
        + stableswap_dir(R1, R0, r1, r0, u1, u0, mu1, mu0, n1, A, Dinv, gam, d1, l0);
+    D[0] = d0; D[1] = d1; L[0] = l0; L[1] = l1;
+}
+
+// Two-coin Curve cryptoswap (v2, twocrypto-ng) pool: scaled balances y_j = p_j x_j (p = price scale times precision),
+// whitepaper amplification A and curve gamma G (not the fee gamma), the invariant of the current reserves D:
+//     K0 = 4 y0 y1 / D^2,   K = A K0 G^2 / (G + 1 - K0)^2,   K D (y0 + y1) + y0 y1 = K D^2 + (D/2)^2.
+// Worked in units of D (u = y / D, the caller passes c_j = p_j / D so u = c x): Phi(u) = K (u0 + u1 - 1) + u0 u1 - 1/4 = 0.
+// Along the curve, with e = 2 u_a - 1, m = 1 - K0 and dl = u_a + u_b - 1 (dl >= 0), the invariant reads K dl = m / 4 and
+// m = e^2 - 4 u_a dl, so m is the root in [0, min(e^2, 1)] of
+//     h(m) = A G^2 (1 - m)(e^2 - m) - u_a m (G + m)^2,       strictly decreasing there (get_y: no closed form),
+// bracketed by [e^2 K(hi) / (K(hi) + u_a), hi], hi = e^2 A / (A + u_a) (m = e^2 K / (K + u_a) with K falling in m).
+// m, dl and u_b - u_a = dl - e are formed from e (exact: 2 u_a - 1 has no rounding where it is small), never as 1 - 4 u0 u1
+// or u0 + u1 - 1, so near the peg they keep their digits against G (1e-5 .. 1e-4 in deployed pools).
+// With K' = dK/dK0 = A G^2 (G + 2 - m) / (G + m)^3 and cc = 1 + 4 dl K', F_a = K + u_b cc, F_b = K + u_a cc, the marginal
+// rate is s = F_a / F_b, s - 1 = cc (u_b - u_a) / F_b.  Tendering a pays iff gamma mu_b s(R) > mu_a with mu = nu / c; the
+// optimal post-trade balance solves log s(u_a) = log(mu_a / (gamma mu_b)) by the stableswap_dir scheme in t = log u_a,
+// with dlog s/dt = u_a (Phi_aa - 2 s Phi_ab + s^2 Phi_bb) / F_a, the curvature grouped so the large K' terms cancel
+// analytically: 8 K' (-(s - 1)(d - (s - 1) u_a) - s dl) + 16 K'' dl (d - (s - 1) u_a)^2 - 2 s, d = u_b - u_a.
+// hc = -nu_a X_a / (gamma dlog s/dt), as for StableSwap.  Fixed iteration caps, scalar arguments only (no stack);
+// shared by the per-thread solver and k_eval_crypto (cfmm_kernels.cu).
+
+// The curve point at u_a: u_b, dl, m and K, K', K''.  ag2 = A G^2.
+CFMM_HD inline void crypto_point(double ua, double A, double G, double ag2, double& ub, double& dl, double& m, double& K,
+                                 double& K1, double& K2) {
+    const double e = 2.0 * ua - 1.0, e2 = e * e;
+    const double mtop = fmin(e2, 1.0);
+    double hi = fmin(e2 * A / (A + ua), mtop);
+    const double gh = G + hi, Kh = ag2 * (1.0 - hi) / (gh * gh);
+    double lo = fmin(e2 * Kh / (Kh + ua), hi);
+    m = hi;
+    if (hi > 0.0) {
+        // safeguarded Newton on h inside [lo, hi] (h falls: h(lo) >= 0 >= h(hi)), from the upper end
+        m = 0.5 * (lo + hi);
+        for (int it = 0; it < 60; ++it) {
+            const double g = G + m;
+            const double f = ag2 * (1.0 - m) * (e2 - m) - ua * m * g * g;
+            if (f > 0.0) lo = m; else hi = m;
+            if (f == 0.0 || !(hi - lo > 2e-16 * m)) break;
+            const double df = -ag2 * ((1.0 - m) + (e2 - m)) - ua * g * (G + 3.0 * m);
+            double mn = m - f / df;
+            if (!(mn > lo && mn < hi)) mn = 0.5 * (lo + hi);
+            if (fabs(mn - m) <= 1e-16 * m) { m = mn; break; }
+            m = mn;
+        }
+    }
+    const double g = G + m, g2 = g * g;
+    K = ag2 * (1.0 - m) / g2;
+    K1 = ag2 * (G + 2.0 - m) / (g2 * g);
+    K2 = ag2 * (4.0 * G + 6.0 - 2.0 * m) / (g2 * g2);
+    // dl = m / (4K) where m is close to e^2 (e^2 - m cancels there), else (e^2 - m) / (4 u_a)
+    dl = (m > 0.5 * e2) ? m / (4.0 * K) : (e2 - m) / (4.0 * ua);
+    ub = ua <= 1.0 ? (1.0 - ua) + dl : (1.0 - m) / (4.0 * ua);
+}
+
+// log s - logq at u_a = exp(t) on the curve, and its derivative in t; ub out
+CFMM_HD inline double crypto_phi(double t, double A, double G, double ag2, double logq, double* dphi, double& ub) {
+    const double ua = exp(t);
+    double dl, m, K, K1, K2;
+    crypto_point(ua, A, G, ag2, ub, dl, m, K, K1, K2);
+    const double d = dl - (2.0 * ua - 1.0);                             // u_b - u_a
+    const double cc = 1.0 + 4.0 * dl * K1;
+    const double Fa = K + ub * cc, Fb = K + ua * cc;
+    const double sm1 = cc * d / Fb;                                      // s - 1
+    const double s = 1.0 + sm1;
+    const double w = d - sm1 * ua;                                       // u_b - s u_a
+    const double Q = 8.0 * K1 * (-sm1 * w - s * dl) + 16.0 * K2 * dl * w * w - 2.0 * s;
+    *dphi = ua * Q / Fa;
+    return (fabs(sm1) < 0.5 ? log1p(sm1) : log(Fa / Fb)) - logq;
+}
+
+// One direction of cryptoswap_pair: tender a, receive b.  Balances in units of D (ua0 = ca Ra), scaled prices mu = nu / c.
+// Writes the tender Delta_a and the payout Lambda_b and returns hc (all 0 without a trade).
+CFMM_HD inline double crypto_dir(double Ra, double Rb, double ca, double cb, double mua, double mub, double nua, double A,
+                                 double G, double gam, double& Da, double& Lb) {
+    Da = Lb = 0.0;
+    const double ag2 = A * G * G;
+    const double logq = log(mua / (gam * mub));
+    double dphi = 0.0, ub = 0.0;
+    double lo = log(ca * Ra), hi = lo;
+    if (!(crypto_phi(lo, A, G, ag2, logq, &dphi, ub) > 0.0)) return 0.0;   // no trade in this direction
+    for (double step = 1.0; step <= 512.0; step *= 2.0) {               // upper bracket phi(hi) <= 0 (|t| < 700: exp finite)
+        hi = lo + step;
+        if (!(crypto_phi(hi, A, G, ag2, logq, &dphi, ub) > 0.0)) break;
+        lo = hi;
+    }
+    // safeguarded Newton inside [lo, hi], as stableswap_dir
+    double t = lo, dx_old = hi - lo, dx = dx_old;
+    for (int it = 0; it < 100; ++it) {
+        const double f = crypto_phi(t, A, G, ag2, logq, &dphi, ub);
+        if (f > 0.0) lo = t; else hi = t;
+        if (f == 0.0 || !(hi - lo > 4e-16 * (1.0 + fabs(t)))) break;
+        const double tn = t - f / dphi;
+        if (fabs(f) <= 8e-16 * (1.0 + fabs(logq))) {                   // phi at the level of its own rounding
+            if (tn > lo && tn < hi) t = tn;
+            break;
+        }
+        if (!(tn > lo && tn < hi) || fabs(2.0 * f) > fabs(dx_old * dphi)) {
+            dx_old = dx; dx = 0.5 * (hi - lo); t = lo + dx;
+        } else {
+            dx_old = dx; dx = tn - t; t = tn;
+        }
+        if (fabs(dx) <= 1e-15 * (1.0 + fabs(t))) break;
+    }
+    crypto_phi(t, A, G, ag2, logq, &dphi, ub);
+    const double Xa = fmax(exp(t) / ca, Ra), Xb = ub / cb;
+    Da = (Xa - Ra) / gam;
+    Lb = fmax(Rb - Xb, 0.0);
+    return dphi < 0.0 ? -nua * Xa / (gam * dphi) : 0.0;
+}
+
+// c_j = p_j / D: the price scales over the invariant of the current reserves; A, G: the whitepaper amplification and gamma
+CFMM_HD inline void cryptoswap_pair(double R0, double R1, double c0, double c1, double A, double G, double gam, double n0,
+                                    double n1, double* D, double* L, double& hc) {
+    const double mu0 = n0 / c0, mu1 = n1 / c1;
+    double d0, l1, d1, l0;
+    hc = crypto_dir(R0, R1, c0, c1, mu0, mu1, n0, A, G, gam, d0, l1)
+       + crypto_dir(R1, R0, c1, c0, mu1, mu0, n1, A, G, gam, d1, l0);
     D[0] = d0; D[1] = d1; L[0] = l0; L[1] = l1;
 }
 
@@ -522,7 +640,10 @@ CFMM_UNROLL
 // LADDER (with STABLE and STABLE_N): also concentrated pools (kind 6) through ladder_pair, their (s, c) in the pool's two
 // w slots, (first record, T) in its two logrw slots and the records in `rec`; cfmm_batch_solve_concentrated runs this
 // fourth instance.  The other instances give problems with such pools status 3.
-template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false>
+// CRYPTO (with all three): also two-coin cryptoswap pools (kind 8) through cryptoswap_pair, c_j = p_j / D in the pool's
+// two w slots and (A, G) in its two logrw slots; cfmm_batch_solve_cryptoswap runs this fifth instance.  The other
+// instances give problems with such pools status 3.
+template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane,
                                const double* rec = nullptr) {
@@ -539,7 +660,16 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
         const int k = (int)(P.pool_ptr[i + 1] - off);
         const double gam = P.gamma[i];
         double D[KMAX], L[KMAX];
-        if (LADDER && P.kind[i] == 6) {                                   // (s, c) in w, (first record, T) in logrw
+        if (CRYPTO && P.kind[i] == 8) {                                   // c = p / D in w, (A, G) in logrw
+            double hc = 0.0;
+            cryptoswap_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], P.logrw[off], P.logrw[off + 1], gam,
+                            nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
+            if (Hs && hc != 0.0) {
+                const int t0 = P.tok[off], t1 = P.tok[off + 1];
+                (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
+                (*Hs)[t0 * n + t1] -= hc; (*Hs)[t1 * n + t0] -= hc;
+            }
+        } else if (LADDER && P.kind[i] == 6) {                                   // (s, c) in w, (first record, T) in logrw
             double hc = 0.0;
             ladder_pair(rec + 4 * (int64_t)P.logrw[off], (int64_t)P.logrw[off + 1], (int64_t)P.w[off + 1], P.w[off], gam,
                         nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
@@ -767,7 +897,7 @@ CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL 
 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
 // rec: the concentrated pools' records (LADDER instance only).
-template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false>
+template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0, const double* rec = nullptr) {
     const int n = Q.n;
@@ -787,9 +917,9 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int64_t o = P.pool_ptr[i];
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1;
-        bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6)) || k < 2 || k > KMAX ||
-              ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
-                (LADDER && P.kind[i] == 6)) && k != 2);
+        bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6) && !(CRYPTO && P.kind[i] == 8)) || k < 2 ||
+              k > KMAX || ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
+                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8)) && k != 2);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
     if (bad) {
@@ -816,7 +946,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -862,7 +992,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -887,8 +1017,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -913,8 +1043,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

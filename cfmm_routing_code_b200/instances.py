@@ -416,3 +416,66 @@ def synth_concentrated_market(m, n_tokens, seed, T=(1, 64), frac_ladder=0.5, emp
                    np.concatenate(tok).astype(np.int32), np.concatenate(R), np.concatenate(w), np.concatenate(g),
                    np.concatenate(kd).astype(np.uint8), np.concatenate(amp), None, lad_ptr, rec, sc)
     return hp, p
+
+
+TWOCRYPTO_A_MULTIPLIER = 10000      # twocrypto-ng stores A() = A * N^N * A_MULTIPLIER (N = 2), gamma() as 1e18 fixed point
+
+
+def twocrypto_pool(A_raw, gamma_raw, price_scale, precisions, balances, mid_fee, out_fee, fee_gamma):
+    """A two-coin Curve v2 (twocrypto-ng) pool's on-chain state as this package's 'cryptoswap' pool.
+    A_raw = A(), gamma_raw = gamma() (1e18 fixed point), price_scale = price_scale() (coin 1 in coin 0, 1e18 fixed point),
+    precisions = the contract's (10^(18 - decimals_0), 10^(18 - decimals_1)), balances = balances(0), balances(1) (raw
+    integers), mid_fee / out_fee (1e10 fixed point) and fee_gamma (1e18).  Returns (weights, reserves, gamma): weights =
+    (A, G, p_0, p_1) for HostPools.from_lists, reserves in whole tokens (balance * precision / 1e18) and the fee gamma
+    = 1 - fee at the current state, fee = mid_fee f + out_fee (1 - f), f = fee_gamma / (fee_gamma + 1 - K0),
+    K0 = 4 y0 y1 / (y0 + y1)^2 with y = p * reserves.  The contract charges that fee on the output and moves it with the
+    trade, so this gamma is the pool's fee for small trades only (as for StableSwap pools, instances give the caller's
+    conversion).  A = A_raw / (A_MULTIPLIER * 2^2) and G = gamma_raw / 1e18: the convention of the contract's comments
+    (A_MULTIPLIER = 10000, A() scaled by N^N); it has not been checked against the contract's integer newton_D (see
+    INTEGRATION.md)."""
+    A = float(A_raw) / (TWOCRYPTO_A_MULTIPLIER * 4)
+    G = float(gamma_raw) / 1e18
+    x = np.array([float(balances[0]) * float(precisions[0]), float(balances[1]) * float(precisions[1])]) / 1e18
+    p = np.array([1.0, float(price_scale) / 1e18])
+    y = p * x
+    K0 = 4.0 * y[0] * y[1] / (y[0] + y[1]) ** 2
+    fg = float(fee_gamma) / 1e18
+    f = fg / (fg + 1.0 - K0)
+    fee = (float(mid_fee) * f + float(out_fee) * (1.0 - f)) / 1e10
+    return (A, G, float(p[0]), float(p[1])), (float(x[0]), float(x[1])), 1.0 - fee
+
+
+def synth_crypto_market(m, n_tokens, seed, frac_crypto=0.4, far=0.5, mispricing=0.02, T=(1, 16)):
+    """A market of two-coin cryptoswap pools beside every other kind: a frac_crypto share of m pools are cryptoswap pools
+    on random token pairs (A in {2.5 .. 400}, curve gamma in {1e-5 .. 2e-2}, fees 0.05 .. 0.45 %), value-balanced within a
+    few percent; the price scale of a `far` share of them sits 20 % .. 4x away from the market price (the pool holds
+    balances far from its peg), the others within 0.5 % of it.  The rest is synth_concentrated_market's mix (constant
+    product, two- to four-coin StableSwap, constant sum, bounded_product ranges, tick ladders of T intervals).
+    Returns (HostPools, prices)."""
+    from .pools import HostPools, KIND_CRYPTOSWAP_HOST
+    rng = np.random.default_rng(seed + 7919)
+    n_cs = int(round(frac_crypto * m))
+    base, p = synth_concentrated_market(m - n_cs, n_tokens, seed, T=T, mispricing=mispricing)
+    a = rng.integers(0, n_tokens, n_cs)
+    b = (a + rng.integers(1, n_tokens, n_cs)) % n_tokens
+    off = rng.random(n_cs) < far
+    sh = np.where(off, np.exp(rng.choice([-1.0, 1.0], n_cs) * rng.uniform(np.log(1.2), np.log(4.0), n_cs)),
+                  np.exp(rng.uniform(-0.005, 0.005, n_cs)))
+    scales = np.stack([p[a], p[b] * sh], 1)                      # the pool's internal price of b in a is off by sh
+    V = np.exp(9.0 + 1.5 * rng.standard_normal(n_cs))
+    R = V[:, None] / scales * np.exp(mispricing * rng.standard_normal((n_cs, 2)))
+    A = np.array([2.5, 10.0, 40.0, 400.0])[rng.integers(0, 4, n_cs)]
+    G = np.array([1e-5, 1.45e-4, 2e-3, 2e-2])[rng.integers(0, 4, n_cs)]
+    gam = np.array([0.9995, 0.9974, 0.9955])[rng.integers(0, 3, n_cs)]
+    m0 = base.m
+    cg = np.concatenate([np.asarray(base.cgam, float), G])
+    hp = HostPools(n_tokens, np.concatenate([base.pool_ptr, base.pool_ptr[-1] + 2 * np.arange(1, n_cs + 1)]).astype(np.int64),
+                   np.concatenate([base.tok_idx, np.stack([a, b], 1).ravel()]).astype(np.int32),
+                   np.concatenate([base.reserves, R.ravel()]), np.concatenate([base.weights, scales.ravel()]),
+                   np.concatenate([base.gamma, gam]),
+                   np.concatenate([base.kind, np.full(n_cs, KIND_CRYPTOSWAP_HOST, np.uint8)]).astype(np.uint8),
+                   np.concatenate([base.amp, A]), None,
+                   np.concatenate([base.lad_ptr, np.full(n_cs, base.lad_ptr[-1], np.int64)]), base.lad_rec,
+                   np.concatenate([base.lad_sc, np.zeros((n_cs, 2))]), cg)
+    assert hp.m == m0 + n_cs
+    return hp, p

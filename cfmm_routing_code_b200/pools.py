@@ -24,6 +24,9 @@ KIND_STABLESWAP_HOST = 4  # StableSwap (Curve), 2..8 coins; rates ride in `weigh
 ANN_MAX = 4e7           # largest StableSwap coefficient A n^n accepted, any coin count (A <= 1e7 for two coins)
 STABLE_ARITY_MAX = 8    # most coins of a StableSwap pool
 KIND_CONCENTRATED_HOST = 6  # concentrated liquidity: a whole Uniswap-v3 tick ladder; records in HostPools.lad_rec
+KIND_CRYPTOSWAP_HOST = 8  # two-coin Curve cryptoswap; price scales ride in `weights`, A in HostPools.amp, gamma in .cgam
+CRYPTO_A_RANGE = (1e-6, 1e4)       # accepted whitepaper A of cryptoswap pools (the concavity of D is checked over it)
+CRYPTO_GAMMA_RANGE = (1e-6, 0.1)   # accepted curve gamma of cryptoswap pools (tests/test_cryptoswap.py checks the corners)
 LADDER_T_MAX = 1 << 20  # most intervals of one concentrated pool (cfmm_small::LADDER_T_MAX)
 
 
@@ -257,6 +260,56 @@ def stableswap_invariant_any(reserves, rates, amp) -> np.ndarray:
     return (stableswap_invariant if n == 2 else stableswap_invariant_n)(reserves, rates, amp)
 
 
+def cryptoswap_invariant(reserves, scales, amp, cgam) -> np.ndarray:
+    """Invariant D of two-coin cryptoswap pools: with y = scales * reserves, K0 = 4 y0 y1 / D^2 and
+    K = A K0 G^2 / (G + 1 - K0)^2 the root D in [2 sqrt(y0 y1), y0 + y1] of
+        f(D) = K D (y0 + y1) + y0 y1 - K D^2 - (D/2)^2.
+    reserves, scales: (m, 2); amp: (m,), the whitepaper A; cgam: (m,), the curve gamma G.  Newton's method on f in D (what
+    Curve's newton_D runs, here in fp64 and in units of y0 + y1, so nothing over- or underflows), from the upper bound
+    D = y0 + y1, kept inside the bracket by a bisection step whenever Newton would leave it; where |y0 - y1| < D, 1 - K0
+    is formed as ((y0 - y1)^2 - (S - D)(S + D)) / D^2, without cancellation near the peg.  A pool stops once a step moves D by at most
+    2 ulp.  Elementwise, each pool's arithmetic in a fixed order: a subset (PoolStore.update_pools) gives the same bits as
+    the whole."""
+    y = np.asarray(reserves, np.float64).reshape(-1, 2) * np.asarray(scales, np.float64).reshape(-1, 2)
+    A = np.asarray(amp, np.float64).reshape(-1)
+    G = np.asarray(cgam, np.float64).reshape(-1)
+    scale = y[:, 0] + y[:, 1]
+    with np.errstate(all="ignore"):
+        y0, y1 = y[:, 0] / scale, y[:, 1] / scale
+        S, P, dy2 = y0 + y1, y0 * y1, (y0 - y1) * (y0 - y1)
+        lo, hi = 2.0 * np.sqrt(P), S.copy()
+        out = S.copy()
+        act = np.arange(len(S))
+        for _ in range(255):
+            if len(act) == 0:
+                break
+            d, a, g, s_, p_ = out[act], A[act], G[act], S[act], P[act]
+            # 1 - K0, from whichever form cancels less: (y0 - y1)^2 and S^2 - D^2 are each below D^2 where |y0 - y1| < D
+            near = dy2[act] < d * d
+            K0 = np.where(near, 0.0, 4.0 * p_ / (d * d))
+            m = np.where(near, (dy2[act] - (s_ - d) * (s_ + d)) / (d * d), 1.0 - K0)
+            K0 = np.where(near, 1.0 - m, K0)
+            gm = g + m
+            K = a * K0 * g * g / (gm * gm)
+            f = K * d * (s_ - d) - 0.25 * m * d * d                        # y0 y1 - D^2 / 4 = -(1 - K0) D^2 / 4
+            # df/dD: dK/dD = K'(K0) dK0/dD, dK0/dD = -2 K0 / D, K'(K0) = A G^2 (G + 2 - m) / (G + m)^3
+            dK = -2.0 * K0 / d * a * g * g * (g + 2.0 - m) / (gm * gm * gm)
+            fp = dK * d * (s_ - d) + K * (s_ - 2.0 * d) - 0.5 * d
+            lo[act] = np.where(f > 0, d, lo[act])
+            hi[act] = np.where(f > 0, hi[act], d)
+            dn = d - f / fp
+            dn = np.where(f == 0, d, np.where((dn > lo[act]) & (dn < hi[act]), dn, 0.5 * (lo[act] + hi[act])))
+            out[act] = dn
+            act = act[~((np.abs(dn - d) <= 4.5e-16 * dn) | (f == 0))]
+    return out * scale
+
+
+def _crypto_groups(kind, pool_ptr):
+    """(pool ids, (m, 2) CSR offsets) of the cryptoswap pools"""
+    cs = np.nonzero(np.asarray(kind) == KIND_CRYPTOSWAP_HOST)[0]
+    return cs, np.asarray(pool_ptr, np.int64)[cs][:, None] + np.arange(2)
+
+
 def _stable_groups(kind, pool_ptr):
     """(n, pool ids, (m, n) CSR offsets) of the StableSwap pools, one entry per coin count"""
     ss = np.nonzero(np.asarray(kind) == KIND_STABLESWAP_HOST)[0]
@@ -285,6 +338,9 @@ class HostPools:
     lad_ptr: Optional[np.ndarray] = None   # int64 [m+1]
     lad_rec: Optional[np.ndarray] = None   # f64 [n_records, 4]
     lad_sc: Optional[np.ndarray] = None    # f64 [m, 2]
+    # cryptoswap pools (kind 8): the curve gamma G (the whitepaper A is in amp, the invariant D in inv, the price scales in
+    # weights); 0 on other kinds.  None: all zero.
+    cgam: Optional[np.ndarray] = None      # f64 [m]
 
     def __post_init__(self):
         m = len(self.gamma)
@@ -296,10 +352,15 @@ class HostPools:
             self.lad_sc = np.zeros((m, 2))
         if self.amp is None:
             self.amp = np.zeros(m)
+        if self.cgam is None:
+            self.cgam = np.zeros(m)
         if self.inv is None:
             self.inv = np.zeros(m)
             for _, ss, off in _stable_groups(self.kind, self.pool_ptr):
                 self.inv[ss] = stableswap_invariant_any(self.reserves[off], self.weights[off], self.amp[ss])
+            cs, off = _crypto_groups(self.kind, self.pool_ptr)
+            if len(cs):
+                self.inv[cs] = cryptoswap_invariant(self.reserves[off], self.weights[off], self.amp[cs], self.cgam[cs])
 
     @property
     def m(self) -> int:
@@ -316,12 +377,16 @@ class HostPools:
         whitepaper A.  And 'concentrated' (a whole Uniswap-v3 tick ladder as one pool): weights[i] = (price, bounds,
         liquidity) with the current price and the T + 1 price bounds in token 1 per token 0 (the caller's token units;
         instances.v3_ladder converts on-chain state), T >= 1 liquidities >= 0 (not all 0), at most LADDER_T_MAX; reserves[i]
-        must be None: the real reserves are derived (ladder_state)."""
+        must be None: the real reserves are derived (ladder_state).  And 'cryptoswap' (a two-coin Curve v2 pool, twocrypto-ng):
+        weights[i] = (A, G, p_0, p_1) with A the whitepaper amplification (K -> A K0 as G -> inf, StableSwap's A), G the
+        curve's gamma (not the fee) and p_j the price scale times the precision of coin j (only p_0 / p_1 matters);
+        A in CRYPTO_A_RANGE, G in CRYPTO_GAMMA_RANGE.  instances.twocrypto_pool converts a contract's state."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
         ptr = [0]; idx: List[int] = []; res: List[float] = []; wts: List[float] = []; kd: List[int] = []
         amp = np.zeros(m)
+        cgam = np.zeros(m)
         lad = {}                                         # concentrated pool -> its records and price
         for i, l in enumerate(local_indices):
             k = len(l)
@@ -362,6 +427,12 @@ class HostPools:
                                      "(A, r_0, ..., r_{n-1})")
                 _check_stableswap(p[0], p[1:], reserves[i], f"pool {i}: ")
                 kd.append(KIND_STABLESWAP_HOST); wts += [float(x) for x in p[1:]]; amp[i] = p[0]
+            elif kinds[i] == "cryptoswap":
+                p = None if (weights is None or weights[i] is None) else np.asarray(weights[i], float).reshape(-1)
+                if k != 2 or p is None or len(p) != 4:
+                    raise ValueError(f"pool {i}: cryptoswap needs 2 tokens and weights[i] = (A, gamma, p_0, p_1)")
+                _check_cryptoswap(p[0], p[1], p[2:], reserves[i], f"pool {i}: ")
+                kd.append(KIND_CRYPTOSWAP_HOST); wts += [float(x) for x in p[2:]]; amp[i] = p[0]; cgam[i] = p[1]
             elif kinds[i] in ("geomean", "product"):
                 w = np.ones(k) if (weights is None or weights[i] is None) else np.asarray(weights[i], float)
                 if len(w) != k or np.any(w <= 0):
@@ -386,7 +457,7 @@ class HostPools:
         return HostPools(int(n_tokens), np.asarray(ptr, np.int64), np.asarray(idx, np.int32),
                          res, np.asarray(wts, np.float64),
                          np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp, None, lad_ptr,
-                         np.concatenate(recs) if recs else None, lad_sc)
+                         np.concatenate(recs) if recs else None, lad_sc, cgam)
 
     @staticmethod
     def from_pairs(n_tokens, idx, reserves, gamma) -> "HostPools":
@@ -430,6 +501,14 @@ class HostPools:
             D = np.asarray(self.inv, float)[ss]
             if not bool(np.all(np.isfinite(D) & (D > 0))):
                 raise ValueError("stableswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
+        cs, off = _crypto_groups(self.kind, self.pool_ptr)
+        if len(cs):
+            if np.any(np.diff(self.pool_ptr)[cs] != 2):
+                raise ValueError("cryptoswap pools must have 2 tokens")
+            _check_cryptoswap(self.amp[cs], np.asarray(self.cgam, float)[cs], self.weights[off], self.reserves[off])
+            D = np.asarray(self.inv, float)[cs]
+            if not bool(np.all(np.isfinite(D) & (D > 0))):
+                raise ValueError("cryptoswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
 
 
     def _validate_ladders(self):
@@ -471,6 +550,20 @@ class HostPools:
             raise ValueError("concentrated (s, c): s must lie in [b_0, b_T] and c be its interval")
 
 
+def _check_cryptoswap(A, G, scales, reserves, where=""):
+    """The value rules of cryptoswap pools: A in CRYPTO_A_RANGE, G in CRYPTO_GAMMA_RANGE (the domain over which the
+    concavity of D is checked), price scales and reserves finite and > 0."""
+    A, G, p, R = (np.asarray(x, float) for x in (A, G, scales, reserves))
+    if not bool(np.all((A >= CRYPTO_A_RANGE[0]) & (A <= CRYPTO_A_RANGE[1]))):
+        raise ValueError(f"{where}cryptoswap amplification A must lie in [{CRYPTO_A_RANGE[0]:g}, {CRYPTO_A_RANGE[1]:g}]")
+    if not bool(np.all((G >= CRYPTO_GAMMA_RANGE[0]) & (G <= CRYPTO_GAMMA_RANGE[1]))):
+        raise ValueError(f"{where}cryptoswap curve gamma must lie in [{CRYPTO_GAMMA_RANGE[0]:g}, {CRYPTO_GAMMA_RANGE[1]:g}]")
+    if not bool(np.all(np.isfinite(p) & (p > 0))):
+        raise ValueError(f"{where}cryptoswap price scales must be finite and > 0")
+    if not bool(np.all(np.isfinite(R) & (R > 0))):
+        raise ValueError(f"{where}cryptoswap reserves must be finite and > 0")
+
+
 def _check_stableswap(A, rates, reserves, where=""):
     """The value rules of StableSwap pools of n coins (the last axis of rates): A finite, A > 0 and A n^n <= ANN_MAX
     (A <= 1e7 at n = 2), rates finite and > 0, reserves finite and > 0."""
@@ -496,7 +589,8 @@ class PoolUpdate:
     prices: Optional[np.ndarray] = None   # f64 [n] new prices of concentrated pools, or None
     ladders: Optional[list] = None        # [n] new (price, bounds f64, liquidity f64) of concentrated pools, or None
     amp: Optional[np.ndarray] = None      # f64 [n] new amplifications A of StableSwap pools, or None
-    rates: Optional[np.ndarray] = None    # f64 [nnz] new rates of StableSwap pools at `slots`, or None
+    rates: Optional[np.ndarray] = None    # f64 [nnz] new rates (price scales) of StableSwap (cryptoswap) pools at `slots`
+    curve_gamma: Optional[np.ndarray] = None   # f64 [n] new curve gammas of cryptoswap pools, or None
 
 
 def _pool_rows(vals, n, ar, what):
@@ -514,7 +608,7 @@ def _pool_rows(vals, n, ar, what):
 
 
 def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarray, pool_ids, reserves=None,
-                      fees=None, prices=None, ladders=None, amp=None, rates=None) -> PoolUpdate:
+                      fees=None, prices=None, ladders=None, amp=None, rates=None, curve_gamma=None) -> PoolUpdate:
     """Host checks of PoolStore.update_pools, on the problem's CSR arrays (pool_ptr, kind, weights as in HostPools).
     pool_ids: global pool indices, distinct and in range; reserves[k]: the new reserve vector of pool pool_ids[k] with the
     pool's arity (a row of the reference's `reserves` literal; an (n, k) array when all pools have arity k); fees[k]: its
@@ -523,7 +617,9 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
     takes no reserves (they are derived from its price).  ladders[k]: the new (price, bounds, liquidity) of concentrated
     pool pool_ids[k], the triple of HostPools.from_lists' weights[i] (T may differ from the pool's old T; the rules of
     from_lists); not together with prices=.  amp[k]: the new whitepaper A of StableSwap pool pool_ids[k], rates[k]: its new
-    rate vector (the pool's arity; an (n, k) array as for reserves), under the rules of from_lists.
+    rate vector (the pool's arity; an (n, k) array as for reserves), under the rules of from_lists.  For cryptoswap pools
+    amp[k] is the new whitepaper A, rates[k] the new price scales (p_0, p_1), curve_gamma[k] the new curve gamma (cryptoswap
+    pools only); amp= and rates= may not mix StableSwap and cryptoswap pools in one call.
     Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order."""
     m = len(pool_ptr) - 1
     ids = np.asarray(pool_ids)
@@ -531,8 +627,8 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
         raise ValueError("pool_ids must be a 1-d sequence of integer pool indices")
     ids = ids.astype(np.int64)
     n = len(ids)
-    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates)):
-        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates or several")
+    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates, curve_gamma)):
+        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates, curve_gamma or several")
     if n and (ids.min() < 0 or ids.max() >= m):
         raise ValueError(f"pool id out of range [0, {m})")
     conc = np.asarray(kind)[ids] == KIND_CONCENTRATED_HOST
@@ -591,10 +687,27 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             _check_ladder(t[0], t[1], t[2], f"ladders[{k}]: ")
             lad.append((float(np.asarray(t[0], np.float64).reshape(-1)[0]), np.asarray(t[1], np.float64).reshape(-1),
                         np.asarray(t[2], np.float64).reshape(-1)))
-    A = W = None
-    if amp is not None or rates is not None:
+    A = W = CG = None
+    crypto = np.asarray(kind)[ids] == KIND_CRYPTOSWAP_HOST
+    if curve_gamma is not None:
+        if not bool(np.all(crypto)):
+            raise ValueError("curve_gamma= applies to cryptoswap pools only")
+        CG = np.ascontiguousarray(curve_gamma, np.float64).reshape(-1)
+        if len(CG) != n:
+            raise ValueError("curve_gamma: one per pool")
+    if n and (amp is not None or rates is not None or curve_gamma is not None) and bool(np.all(crypto)):
+        if amp is not None:
+            A = np.ascontiguousarray(amp, np.float64).reshape(-1)
+            if len(A) != n:
+                raise ValueError("amp: one per pool")
+        if rates is not None:
+            W = _pool_rows(rates, n, ar, "rates")
+        _check_cryptoswap(np.full(n, CRYPTO_A_RANGE[0]) if A is None else A,
+                          np.full(n, CRYPTO_GAMMA_RANGE[0]) if CG is None else CG,
+                          np.ones((n, 2)) if W is None else W.reshape(n, 2), np.ones((n, 2)))
+    elif amp is not None or rates is not None:
         if not bool(np.all(np.asarray(kind)[ids] == KIND_STABLESWAP_HOST)):
-            raise ValueError("amp= and rates= apply to StableSwap pools only")
+            raise ValueError("amp= and rates= apply to StableSwap or cryptoswap pools only (not both in one call)")
         if amp is not None:
             A = np.ascontiguousarray(amp, np.float64).reshape(-1)
             if len(A) != n:
@@ -606,7 +719,7 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             _check_stableswap(np.ones(len(sel)) if A is None else A[sel],
                               np.ones((len(sel), k)) if W is None else W[first[sel][:, None] + np.arange(k)],
                               np.ones((len(sel), k)))
-    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W)
+    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W, CG)
 
 
 class BucketSpec:
@@ -690,6 +803,11 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         if np.any(ar[cl] != 2):
             raise ValueError("concentrated pools must have 2 tokens")
         keys.append((_lib.KIND_CONCENTRATED, 2, np.nonzero(cl)[0]))
+    cs = hp.kind == KIND_CRYPTOSWAP_HOST
+    if cs.any():
+        if np.any(ar[cs] != 2):
+            raise ValueError("cryptoswap pools must have 2 tokens")
+        keys.append((_lib.KIND_CRYPTOSWAP, 2, np.nonzero(cs)[0]))
     gm = (hp.kind == KIND_GEOMEAN_HOST) & ~is_cp
     for k in np.unique(ar[gm]).tolist():
         if k < 2 or k > 32:
@@ -748,6 +866,10 @@ class DeviceBucket:
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
             AD = np.stack([hp.amp[spec.sel], hp.inv[spec.sel]])
             self.logrw = torch.as_tensor(_padded(AD, self.stride, 1.0), **f64)
+        if self.kind == _lib.KIND_CRYPTOSWAP:              # price scales in the weights slot, (A, G, D) in three logrw rows
+            self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
+            AGD = np.stack([hp.amp[spec.sel], np.asarray(hp.cgam, np.float64)[spec.sel], hp.inv[spec.sel]])
+            self.logrw = torch.as_tensor(_padded(AGD, self.stride, 1.0), **f64)
         if self.kind == _lib.KIND_CONCENTRATED:            # this bucket's records in the weights slot, (s, c, first, T) in logrw
             sel = spec.sel
             first = np.asarray(hp.lad_ptr, np.int64)[sel]
@@ -781,11 +903,13 @@ class DeviceBucket:
 
     def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
                      W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None, sc: Optional[np.ndarray] = None,
-                     rates: Optional[np.ndarray] = None, AD: Optional[np.ndarray] = None):
+                     rates: Optional[np.ndarray] = None, AD: Optional[np.ndarray] = None,
+                     cgam: Optional[np.ndarray] = None):
         """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
         Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__;
         StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,), or, when
         their A or rates change, the new rates (arity, n) in the weights rows and AD = (A, D) (2, n) in logrw rows 0-1;
+        cryptoswap pools likewise, with their curve gammas cgam (n,), and AD = (A, G, D) (3, n) in logrw rows 0-2;
         concentrated pools get their new (s, c) from sc (2, n), with R their derived reserves (ladder_state)."""
         f64 = dict(dtype=torch.float64, device=self._device)
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
@@ -796,12 +920,15 @@ class DeviceBucket:
             if self.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N):
                 if AD is None:
                     self.logrw[1, li] = torch.as_tensor(stableswap_invariant_any(R.T, W.T, amp), **f64)
+            elif self.kind == _lib.KIND_CRYPTOSWAP:
+                if AD is None:
+                    self.logrw[2, li] = torch.as_tensor(cryptoswap_invariant(R.T, W.T, amp, cgam), **f64)
             elif self.kind == _lib.KIND_GEOMEAN:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
         if rates is not None:
             self.weights[:, li] = torch.as_tensor(rates, **f64)
         if AD is not None:
-            self.logrw[:2, li] = torch.as_tensor(AD, **f64)
+            self.logrw[:len(AD), li] = torch.as_tensor(AD, **f64)
         if gamma is not None:
             self.gamma[li] = torch.as_tensor(gamma, **f64)
 
@@ -1279,7 +1406,8 @@ class PoolStore:
         # borrowed from hp and never written: update_pools(amp=, rates=) copies weights and amp first, and ladders live in
         # a LadderSlab over hp's records (made at the first update that needs them)
         self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets / rates
-        self._amp_host = hp.amp                                          # StableSwap amplification
+        self._amp_host = hp.amp                                          # StableSwap / cryptoswap amplification
+        self._cgam_host = hp.cgam                                        # cryptoswap curve gamma
         self._own_stable = False                                         # weights / amp are this store's copies
         self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records
         self._lad = None                                                 # LadderSlab
@@ -1349,6 +1477,7 @@ class PoolStore:
             n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED
                         else 80 if b.kind == _lib.KIND_CONCENTRATED
                         else 64 if b.kind == _lib.KIND_STABLESWAP
+                        else 72 if b.kind == _lib.KIND_CRYPTOSWAP
                         else 20 * b.arity + 24 if b.kind == _lib.KIND_STABLESWAP_N else 32)
         return n + 16 * self.n_tokens + 8
 
@@ -1463,7 +1592,8 @@ class PoolStore:
             self._lad = LadderSlab(*self._lad_host)
         return self._lad
 
-    def update_pools(self, pool_ids, reserves=None, fees=None, prices=None, ladders=None, amp=None, rates=None):
+    def update_pools(self, pool_ids, reserves=None, fees=None, prices=None, ladders=None, amp=None, rates=None,
+                     curve_gamma=None):
         """Set new reserves, fees, prices, ladders, amplifications and / or rates of some pools in place: the store then
         equals, bit for bit, a PoolStore built from a HostPools of the updated literals, without re-uploading the pools or
         rebuilding the blocked layout (which depends on the token ids only).  pool_ids: global pool indices (the order of
@@ -1474,6 +1604,8 @@ class PoolStore:
         pools only): its new whitepaper A / rate vector (a ramp of A, a moved rate oracle); D is then recomputed with
         stableswap_invariant_any from the pool's reserves after the call (the new ones if reserves= is given, else its
         current ones, read back from the device), and later reserves= updates use the new A and rates.
+        Cryptoswap pools take reserves= and fees= (D recomputed with cryptoswap_invariant), rates= (new price scales: a
+        repeg of price_scale), amp= and curve_gamma= (a step of ramp_A_gamma); D is then recomputed as for StableSwap.
         Concentrated pools take prices= (prices[k]: the new price of pool pool_ids[k], token 1 per token 0) instead of
         reserves=, which raises for them: their (s, c) and real reserves are recomputed with ladder_state, the function
         HostPools uses.  ladders[k] = (price, bounds, liquidity) (concentrated pools only, not with prices=): the pool's
@@ -1495,7 +1627,7 @@ class PoolStore:
             store.update_pools(ids, reserves=new_R, fees=new_gamma)
             res = solve_pools(hp, utility, store=store, nu0=res.nu)"""
         u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees, prices,
-                              ladders, amp, rates)
+                              ladders, amp, rates, curve_gamma)
         bi, loc = self._pool_map()
         owner = bi[u.ids]
         plan = []
@@ -1518,14 +1650,20 @@ class PoolStore:
                 rec, cnt, s, c, x, y = new_ladders([u.ladders[j] for j in e.tolist()])
                 n_total = b.n_rec + int(cnt.sum()) - int((self._ladders().T[ids] + 1).sum())
                 lad = (rec, cnt, np.stack([s, c, x, y], 1), n_total)
-            if u.amp is not None or u.rates is not None:   # StableSwap pools only (checked): D of the reserves after the call
+            if u.amp is not None or u.rates is not None or u.curve_gamma is not None:
+                # StableSwap or cryptoswap pools only (checked): D of the reserves after the call
                 A = u.amp[e] if u.amp is not None else self._amp_host[ids]
                 rt = u.rates[rs] if u.rates is not None else self._weights_host[u.slots[rs]]
                 Rd = R if R is not None else b.reserves[:, torch.as_tensor(loc[ids], device=self.device)].cpu().numpy()
-                D = stableswap_invariant_any(Rd.T, rt.T, A)
+                if b.kind == _lib.KIND_CRYPTOSWAP:
+                    G = u.curve_gamma[e] if u.curve_gamma is not None else self._cgam_host[ids]
+                    D = cryptoswap_invariant(Rd.T, rt.T, A, G)
+                    AD = np.stack([A, G, D])
+                else:
+                    D = stableswap_invariant_any(Rd.T, rt.T, A)
+                    AD = np.stack([A, D])
                 if not bool(np.all(np.isfinite(D) & (D > 0))):
-                    raise ValueError("stableswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
-                AD = np.stack([A, D])
+                    raise ValueError("invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
             plan.append((b, loc[ids], R, g, rs, ids, sc, lad, rt, AD))
         # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
         rebuilt = 0
@@ -1538,8 +1676,10 @@ class PoolStore:
             if lad is not None:
                 b.splice_ladders(self.lib, l, lad[0], lad[1], lad[2], lad[3], self._stream())
             W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None and AD is None) else None
-            amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) else None
-            b.write_update(l, R, g, W, amp_, sc, None if u.rates is None else rt, AD)
+            amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N,
+                                                     _lib.KIND_CRYPTOSWAP) else None
+            cg_ = self._cgam_host[ids] if b.kind == _lib.KIND_CRYPTOSWAP else None
+            b.write_update(l, R, g, W, amp_, sc, None if u.rates is None else rt, AD, cg_)
         # the store's host state, once the device holds the update
         for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:
             if lad is not None:
@@ -1547,8 +1687,11 @@ class PoolStore:
             if AD is not None:
                 if not self._own_stable:
                     self._weights_host, self._amp_host = self._weights_host.copy(), self._amp_host.copy()
+                    self._cgam_host = self._cgam_host.copy()
                     self._own_stable = True
                 self._amp_host[ids] = AD[0]
+                if b.kind == _lib.KIND_CRYPTOSWAP:
+                    self._cgam_host[ids] = AD[1]
                 self._weights_host[u.slots[rs]] = rt
         torch.cuda.synchronize(self.device)
         return rebuilt

@@ -58,7 +58,16 @@ enum {
                               exact in f64.  reserves [2][stride] = the real reserves (x, y) at s (not read by the
                               evaluation).  hcoef is per pool, as for every pair kind: the liquidity of the interval the
                               trade ends in (at an exact bound, the one above it; 0 past either end) times
-                              sqrt(nu0 nu1 / gamma) / 2.  Smooth between bounds: no theta_bar                        */
+                              sqrt(nu0 nu1 / gamma) / 2.  Smooth between bounds: no theta_bar                        */,
+    CFMM_KIND_CRYPTOSWAP = 8  /* two-coin Curve cryptoswap (v2, twocrypto-ng): scaled balances y_j = p_j x_j (p = price
+                              scale times precision), K0 = 4 y0 y1 / D^2, K = A K0 G^2 / (G + 1 - K0)^2, and the pool
+                              keeps D(y) >= D(R) for the root D of K D (y0 + y1) + y0 y1 = K D^2 + (D/2)^2 with
+                              2 sqrt(y0 y1) <= D <= y0 + y1.  Not in the reference; arity 2.  weights [2][stride] = the
+                              price scales (p0, p1) > 0 (only their ratio matters); logrw [3][stride]: slot 0 = A (the
+                              whitepaper amplification: K -> A K0 as G -> inf, StableSwap's A), slot 1 = G (the curve's
+                              gamma, not the fee), slot 2 = D of the current reserves.  hcoef is per pool, as for every
+                              pair kind.  Smooth: no theta_bar.  (7 is not a kind: cfmm_arb_eval returns CFMM_E_KIND
+                              for it, as for any other unknown kind.)                                                 */
 };
 
 enum {
@@ -318,13 +327,17 @@ typedef struct cfmm_csr_pools {
     const double* reserves;    /* [nnz]  arbitrage.py:14-20                                          */
     const double* weights;     /* [nnz]  normalised like cp.geo_mean(p=...), arbitrage.py:65; 0 on constant-sum pools;
                                          offsets of bounded products; rates of StableSwap pools; concentrated
-                                         pools: the sqrt price s at the first slot, c at the second     */
+                                         pools: the sqrt price s at the first slot, c at the second;
+                                         cryptoswap pools: p_j / D, the price scales over the invariant
+                                         of the reserves (u = weights * reserves in units of D)         */
     const double* logrw;       /* [nnz]  log(reserves / weights) (unused on constant-sum pools); StableSwap: A at the
                                          pool's first slot, D at its second; concentrated pools: the index of
-                                         the first record at the first slot, T at the second           */
+                                         the first record at the first slot, T at the second; cryptoswap
+                                         pools: A at the first slot, the curve gamma G at the second    */
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
     const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP |
-                                            CFMM_KIND_CONCENTRATED, else weighted geometric mean     */
+                                            CFMM_KIND_CONCENTRATED | CFMM_KIND_CRYPTOSWAP, else weighted
+                                            geometric mean                                           */
 } cfmm_csr_pools;
 
 typedef struct cfmm_batch {
@@ -372,6 +385,12 @@ int cfmm_batch_solve_stableswap_n(const cfmm_csr_pools* pools, const cfmm_batch*
  * NULL.  A fourth kernel instance, so the others keep their registers.  Same limits and workspace. */
 int cfmm_batch_solve_concentrated(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
                                   const cfmm_batch_params* prm, void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_CRYPTOSWAP pools (two coins; the CSR layout above: p_j / D in the
+ * weights, (A, G) in logrw), beside every kind cfmm_batch_solve_concentrated takes (the four entry points above give
+ * their problems status 3).  records: as for cfmm_batch_solve_concentrated, and may be NULL when the pool set has no
+ * concentrated pools.  A fifth kernel instance, so the others keep their registers.  Same limits and workspace. */
+int cfmm_batch_solve_cryptoswap(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
+                                const cfmm_batch_params* prm, void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
