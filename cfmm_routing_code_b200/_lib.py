@@ -10,7 +10,7 @@ import os
 from . import build as _build
 
 KIND_PRODUCT, KIND_SUM, KIND_GEOMEAN, KIND_BOUNDED, KIND_STABLESWAP, KIND_STABLESWAP_N, KIND_CONCENTRATED = 0, 1, 2, 3, 4, 5, 6
-KIND_CRYPTOSWAP = 8
+KIND_CRYPTOSWAP, KIND_CRYPTOSWAP_3 = 8, 9
 
 _ERRORS = {
     -1: "CFMM_E_NULL (required pointer is NULL)",
@@ -165,6 +165,8 @@ def load(build_if_missing: bool = True):
     lib.cfmm_batch_solve_concentrated.restype = C.c_int
     lib.cfmm_batch_solve_cryptoswap.argtypes = lib.cfmm_batch_solve_concentrated.argtypes
     lib.cfmm_batch_solve_cryptoswap.restype = C.c_int
+    lib.cfmm_batch_solve_tricrypto.argtypes = lib.cfmm_batch_solve_concentrated.argtypes
+    lib.cfmm_batch_solve_tricrypto.restype = C.c_int
     lib.cfmm_allreduce_ll.argtypes = [vp, vp, i32, i32, i32, i64, i64, vp, C.c_uint64, vp]
     lib.cfmm_allreduce_ll.restype = C.c_int
     lib.cfmm_sum_update_multipliers.argtypes = [C.POINTER(Bucket), vp, vp, vp, vp]

@@ -69,18 +69,26 @@ class CsrStore:
             self.logrw[first + 1] = torch.as_tensor((lp[cl + 1] - lp[cl] - 1).astype(np.float64), device=dev)
             self.records = torch.as_tensor(np.ascontiguousarray(hp.lad_rec, np.float64).reshape(-1), device=dev)
         cs = np.nonzero(np.asarray(hp.kind) == KIND_CRYPTOSWAP_HOST)[0]
+        ptr = np.asarray(hp.pool_ptr, np.int64)
+        c3 = cs[ptr[cs + 1] - ptr[cs] == 3]
         self.has_crypto = bool(len(cs))              # -> cfmm_batch_solve_cryptoswap (a fifth instance)
+        self.has_crypto3 = bool(len(c3))             # -> cfmm_batch_solve_tricrypto (a sixth instance)
         if len(cs):                                  # cryptoswap pools: p_j / D in the w slots, (A, G) in logrw
-            first = np.asarray(hp.pool_ptr, np.int64)[cs]
+            first = ptr[cs]
             Dv = np.asarray(hp.inv, np.float64)[cs]
             W = np.asarray(hp.weights, np.float64)
             fd = torch.as_tensor(first, device=dev)
             self.w[fd] = torch.as_tensor(W[first] / Dv, device=dev)
             self.w[fd + 1] = torch.as_tensor(W[first + 1] / Dv, device=dev)
+            if len(c3):                              # the third coin of the three-coin pools
+                self.w[torch.as_tensor(ptr[c3] + 2, device=dev)] = torch.as_tensor(W[ptr[c3] + 2] / np.asarray(hp.inv)[c3],
+                                                                                   device=dev)
             self.logrw[fd] = torch.as_tensor(np.asarray(hp.amp, np.float64)[cs], device=dev)
             self.logrw[fd + 1] = torch.as_tensor(np.asarray(hp.cgam, np.float64)[cs], device=dev)
         self.gamma = torch.as_tensor(np.ascontiguousarray(hp.gamma, np.float64), device=dev)
-        self.kind = torch.as_tensor(np.ascontiguousarray(hp.kind, np.uint8), device=dev)
+        kind = np.array(hp.kind, np.uint8)
+        kind[c3] = _lib.KIND_CRYPTOSWAP_3            # three-coin cryptoswap pools are kind 9 in the C ABI
+        self.kind = torch.as_tensor(kind, device=dev)
         self.c_pools = _lib.CsrPools(self.n_tokens, self.m, self.nnz, self.pool_ptr.data_ptr(), self.tok.data_ptr(),
                                      self.R.data_ptr(), self.w.data_ptr(), self.logrw.data_ptr(),
                                      self.gamma.data_ptr(), self.kind.data_ptr())
@@ -131,6 +139,12 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if store.has_crypto3:
+        _lib.check(store.lib.cfmm_batch_solve_tricrypto(C.byref(store.c_pools),
+                                                        store.records.data_ptr() if store.records is not None else None,
+                                                        C.byref(batch), C.byref(prm), work.data_ptr(), st),
+                   "cfmm_batch_solve_tricrypto")
+        return psi, stats, delta, lam
     if store.has_crypto:
         _lib.check(store.lib.cfmm_batch_solve_cryptoswap(C.byref(store.c_pools),
                                                          store.records.data_ptr() if store.records is not None else None,

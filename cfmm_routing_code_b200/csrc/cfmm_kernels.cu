@@ -315,6 +315,47 @@ k_eval_stable_n(long long m, long long ld, int n_tokens, const double* __restric
     block_accumulate(acc, arb);
 }
 
+// three-coin cryptoswap (tricrypto-ng): cfmm_small::cryptoswap3 (a safeguarded Newton solve in m = 1 - K0 around an
+// inner one for the price level, compute-bound), one thread per pool.  scales [3][ld] = the price scales p (the bucket's
+// weights), AGD [3][ld] = (A, G, D) (the bucket's logrw); the kernel passes c = p / D.  hcoef [3][ld] = the edge weights
+// (w01, w02, w12) of the pool's scaled Hessian block, hmask = traded slots.
+template <typename Scatter, bool TRADES, bool HESS>
+__global__ void __launch_bounds__(kThreads)
+k_eval_crypto3(long long m, long long ld, int n_tokens, const double* __restrict__ R, const int* __restrict__ idx,
+               const double* __restrict__ gamma, const double* __restrict__ scales, const double* __restrict__ AGD,
+               const double* __restrict__ nu, double* psi, double* arb, double* delta, double* lambda, double* hcoef,
+               uint32_t* hmask) {
+    extern __shared__ double smem[];
+    Scatter sc{psi};
+    sc.init(smem, n_tokens);
+    double acc = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        const int i0 = idx[i], i1 = idx[ld + i], i2 = idx[2 * ld + i];
+        const double n0 = __ldg(nu + i0), n1 = __ldg(nu + i1), n2 = __ldg(nu + i2);
+        const double Dv = AGD[2 * ld + i];
+        double D[3], L[3], w[3];
+        const uint32_t mask = cfmm_small::cryptoswap3(R[i], R[ld + i], R[2 * ld + i], scales[i] / Dv, scales[ld + i] / Dv,
+                                                      scales[2 * ld + i] / Dv, AGD[i], AGD[ld + i], gamma[i], n0, n1, n2,
+                                                      D, L, w);
+        const double y0 = L[0] - D[0], y1 = L[1] - D[1], y2 = L[2] - D[2];
+        if (TRADES) {
+            delta[i] = D[0]; delta[ld + i] = D[1]; delta[2 * ld + i] = D[2];
+            lambda[i] = L[0]; lambda[ld + i] = L[1]; lambda[2 * ld + i] = L[2];
+        }
+        if (HESS) {
+            hcoef[i] = w[0]; hcoef[ld + i] = w[1]; hcoef[2 * ld + i] = w[2];
+            hmask[i] = mask;
+        }
+        if (y0 != 0.0) sc.add(i0, y0);
+        if (y1 != 0.0) sc.add(i1, y1);
+        if (y2 != 0.0) sc.add(i2, y2);
+        acc += n0 * y0 + n1 * y1 + n2 * y2;
+    }
+    sc.flush(smem, n_tokens);
+    block_accumulate(acc, arb);
+}
+
 // ---------------------------------------------------------------------------------------------
 // TMA-staged variant of the 2-token kernel: persistent CTAs, each walking tiles of kTile pools.
 // One elected thread issues five 1-D bulk copies per tile (cp.async.bulk -> UBLKCP: R0, R1, gamma,
@@ -720,6 +761,58 @@ k_dense_stable_n(long long m, long long ld, int k, int n, const int* __restrict_
     }
 }
 
+// three-coin cryptoswap: Hs = sum_{a<b} w_ab (e_a - e_b)(e_a - e_b)' over the pool's three edges, the weights in hcoef
+// [3][ld] = (w01, w02, w12) (cfmm_small::cryptoswap3); O(1) per pool.  Pools without a trade (hmask 0) are skipped.
+template <typename Scatter>
+__global__ void __launch_bounds__(kThreads)
+k_hvp_crypto3(long long m, long long ld, int n_tokens, const int* __restrict__ idx, const double* __restrict__ hcoef,
+              const uint32_t* __restrict__ hmask, const double* __restrict__ vt, double* y) {
+    extern __shared__ double smem[];
+    Scatter sc{y};
+    sc.init(smem, n_tokens);
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        if (!hmask[i]) continue;
+        const int t0 = idx[i], t1 = idx[ld + i], t2 = idx[2 * ld + i];
+        const double z0 = __ldg(vt + t0), z1 = __ldg(vt + t1), z2 = __ldg(vt + t2);
+        const double e01 = hcoef[i] * (z0 - z1), e02 = hcoef[ld + i] * (z0 - z2), e12 = hcoef[2 * ld + i] * (z1 - z2);
+        sc.add(t0, e01 + e02);
+        sc.add(t1, e12 - e01);
+        sc.add(t2, -e02 - e12);
+    }
+    sc.flush(smem, n_tokens);
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_diag_crypto3(long long m, long long ld, const int* __restrict__ idx, const double* __restrict__ hcoef,
+               const uint32_t* __restrict__ hmask, double* diag) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        if (!hmask[i]) continue;
+        const double w01 = hcoef[i], w02 = hcoef[ld + i], w12 = hcoef[2 * ld + i];
+        atomicAdd(diag + idx[i], w01 + w02);
+        atomicAdd(diag + idx[ld + i], w01 + w12);
+        atomicAdd(diag + idx[2 * ld + i], w02 + w12);
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_dense_crypto3(long long m, long long ld, int n, const int* __restrict__ idx, const double* __restrict__ hcoef,
+                const uint32_t* __restrict__ hmask, double* H) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        if (!hmask[i]) continue;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            const double w = hcoef[q * ld + i];
+            if (w == 0.0) continue;
+            const long long a = idx[(q == 2 ? 1 : 0) * ld + i], b = idx[(q == 0 ? 1 : 2) * ld + i];
+            atomicAdd(H + a * n + a, w); atomicAdd(H + b * n + b, w);
+            atomicAdd(H + a * n + b, -w); atomicAdd(H + b * n + a, -w);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(kThreads)
 k_sum_update(long long m, long long ld, const double* __restrict__ R, const double* __restrict__ lambda,
              double* thbar, double* move) {
@@ -845,6 +938,39 @@ int launch_crypto(const cfmm_bucket* b, int n_tokens, const double* nu, double* 
             hcoef);
     }
     return check_launch();
+}
+
+// three-coin cryptoswap buckets: the LDG path only, as for two coins
+template <bool TRADES, bool HESS>
+int launch_crypto3(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                   const cfmm_eval_out* out, cudaStream_t st) {
+    const long long m = b->n_pools;
+    double* delta = out ? out->delta : nullptr;
+    double* lambda = out ? out->lambda : nullptr;
+    double* hcoef = out ? out->hcoef : nullptr;
+    uint32_t* hmask = out ? out->hmask : nullptr;
+    if (use_shared(n_tokens, m * 3 / 2)) {
+        const size_t sm = (size_t)n_tokens * sizeof(double);
+        auto kern = k_eval_crypto3<SharedScatter, TRADES, HESS>;
+        allow_smem(kern, sm);
+        kern<<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights,
+                                                    b->logrw, nu, psi, arb, delta, lambda, hcoef, hmask);
+    } else {
+        k_eval_crypto3<GlobalScatter, TRADES, HESS><<<grid_for(m, 8), kThreads, 0, st>>>(
+            m, b->stride, n_tokens, b->reserves, b->tok_idx, b->gamma, b->weights, b->logrw, nu, psi, arb, delta, lambda,
+            hcoef, hmask);
+    }
+    return check_launch();
+}
+
+int dispatch_crypto3(const cfmm_bucket* b, int n_tokens, const double* nu, double* psi, double* arb,
+                     const cfmm_eval_out* out, cudaStream_t st) {
+    const bool trades = out && out->delta && out->lambda;
+    const bool hess = out && out->hcoef && out->hmask;
+    if (trades && hess) return launch_crypto3<true, true>(b, n_tokens, nu, psi, arb, out, st);
+    if (trades) return launch_crypto3<true, false>(b, n_tokens, nu, psi, arb, out, st);
+    if (hess) return launch_crypto3<false, true>(b, n_tokens, nu, psi, arb, out, st);
+    return launch_crypto3<false, false>(b, n_tokens, nu, psi, arb, out, st);
 }
 
 // n-coin StableSwap buckets: the LDG path only, as for two coins
@@ -993,6 +1119,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 2) return CFMM_E_KIND;
             if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // price scales; (A, G, D)
             break;
+        case CFMM_KIND_CRYPTOSWAP_3:
+            if (b->arity != 3) return CFMM_E_KIND;
+            if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // price scales; (A, G, D)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -1026,6 +1156,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_CONCENTRATED>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_CRYPTOSWAP:
             return dispatch_pair<CFMM_KIND_CRYPTOSWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_CRYPTOSWAP_3:
+            return dispatch_crypto3(b, n_tokens, nu, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP_N:
             switch (b->arity) {
                 case 2: return dispatch_stable_n<2>(b, n_tokens, nu, psi, arb, out, st);
@@ -1072,6 +1204,16 @@ int cfmm_hvp(const cfmm_bucket* b, int32_t n_tokens, const double* hcoef, const 
             k_hvp_stable_n<GlobalScatter><<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, n_tokens,
                                                                                b->tok_idx, hcoef, hmask, vt, y);
         }
+    } else if (b->kind == CFMM_KIND_CRYPTOSWAP_3) {
+        if (!hmask) return CFMM_E_NULL;
+        if (sh) {
+            allow_smem(k_hvp_crypto3<SharedScatter>, sm);
+            k_hvp_crypto3<SharedScatter><<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->tok_idx, hcoef,
+                                                                               hmask, vt, y);
+        } else {
+            k_hvp_crypto3<GlobalScatter><<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, n_tokens, b->tok_idx, hcoef,
+                                                                              hmask, vt, y);
+        }
     } else if (b->kind == CFMM_KIND_GEOMEAN) {
         if (!hmask) return CFMM_E_NULL;
         if (sh) {
@@ -1104,6 +1246,9 @@ int cfmm_hess_diag(const cfmm_bucket* b, int32_t n_tokens, const double* hcoef, 
     if (b->kind == CFMM_KIND_STABLESWAP_N) {
         if (!hmask) return CFMM_E_NULL;
         k_diag_stable_n<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, b->tok_idx, hcoef, hmask, diag);
+    } else if (b->kind == CFMM_KIND_CRYPTOSWAP_3) {
+        if (!hmask) return CFMM_E_NULL;
+        k_diag_crypto3<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->tok_idx, hcoef, hmask, diag);
     } else if (b->kind == CFMM_KIND_GEOMEAN) {
         if (!hmask) return CFMM_E_NULL;
         k_diag_geomean<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, b->tok_idx, b->weights, hcoef, hmask, diag);
@@ -1125,6 +1270,9 @@ int cfmm_hess_dense(const cfmm_bucket* b, int32_t n_tokens, const double* hcoef,
         if (!hmask) return CFMM_E_NULL;
         k_dense_stable_n<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, n_tokens, b->tok_idx, hcoef, hmask,
                                                                H);
+    } else if (b->kind == CFMM_KIND_CRYPTOSWAP_3) {
+        if (!hmask) return CFMM_E_NULL;
+        k_dense_crypto3<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, n_tokens, b->tok_idx, hcoef, hmask, H);
     } else if (b->kind == CFMM_KIND_GEOMEAN) {
         if (!hmask) return CFMM_E_NULL;
         k_dense_geomean<<<grid_for(m, 8), kThreads, 0, st>>>(m, b->stride, b->arity, n_tokens, b->tok_idx, b->weights, hcoef,

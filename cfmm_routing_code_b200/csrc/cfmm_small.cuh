@@ -36,12 +36,13 @@ struct Pools {                       // CSR problem data (device pointers in the
     const int32_t* tok;              // [nnz]   token of every slot            arbitrage.py:6-12
     const double* R;                 // [nnz]   reserves                       arbitrage.py:14-20
     const double* w;                 // [nnz]   normalised weights | 0 on constant-sum pools | virtual offsets (kind 3) |
-                                     //         rates (kind 4) | p_j / D (kind 8)
+                                     //         rates (kind 4) | p_j / D (kinds 8, 9)
     const double* logrw;             // [nnz]   log(R/w) | kind 4: A at the pool's first slot, its invariant D at the second |
-                                     //         kind 8: A, then the curve gamma G
+                                     //         kinds 8, 9: A, then the curve gamma G
     const double* gamma;             // [m]     fees                           arbitrage.py:22-28
     const uint8_t* kind;             // [m]     1 = constant sum; 3 = bounded-liquidity product; 4 = StableSwap (2 coins;
                                      //         2..KMAX in the STABLE_N instance); 8 = two-coin cryptoswap (CRYPTO instance);
+                                     //         9 = three-coin cryptoswap (CRYPTO3 instance);
                                      //         0 or 2 = weighted geometric mean
                                      //         (constant product = equal weights)
 };
@@ -391,6 +392,259 @@ CFMM_HD inline void cryptoswap_pair(double R0, double R1, double c0, double c1, 
     D[0] = d0; D[1] = d1; L[0] = l0; L[1] = l1;
 }
 
+// Three-coin Curve cryptoswap (tricrypto-ng) pool: y_j = p_j x_j, A, G as for two coins, the invariant D of the current
+// reserves.  In units of D (u = y / D, the caller passes c_j = p_j / D): S = sum u, P = prod u, K0 = 27 P,
+// K = A K0 G^2 / (G + 1 - K0)^2, and the pool keeps Phi(u) = K (S - 1) + P - 1/27 >= 0, with dPhi/du_j = K + Q / u_j,
+// Q = P (1 + 27 (S - 1) K'), K' = dK/dK0.  That is the form a + Q / u_j of stableswap_n, so with pi_j = nu_j / c_j the
+// stationary point at the multiplier mu is u_j = clamp(u0_j, Q / (pi_j / (gamma mu) - K), Q / (pi_j / mu - K)) and the
+// pool is idle iff gamma max rho <= min rho, rho_j = pi_j / dPhi/du_j(u0) (flows and edge weights then exactly 0).
+// K and Q are not constants: with m = 1 - K0 the curve gives P = (1 - m) / 27 and S - 1 = m / (27 K), so
+//     K = A G^2 (1 - m) / (G + m)^2,   Q = (G + 3m - 2m^2) / (27 (G + m)),   l = log(Q / K),
+// all functions of m.  At fixed m, with tau = log(pi_min / (gamma K mu)) and dB_j = log(pi_j / pi_min) as in
+// stableswap_n, log u_j = log u0_j + z_j, z_j = max(l - bA_j, 0) + min(l - bB_j, 0), bA_j = log(u0_j expm1(dB_j + tau)),
+// bB_j = log(u0_j expm1(dB_j + log gamma + tau)) (-inf if that expm1 <= 0): the denominators without cancellation.
+// Two conditions close the system:
+//   E1(tau; m) = sum_j z_j - log1p(-m) + sum_j log1p(e0_j) = 0   (P = (1 - m) / 27; e0_j = 3 u0_j - 1),
+//        strictly falling in tau: one safeguarded Newton in log tau per m (crypto3_tau);
+//   r(m) = sum_j e_j - m / (9 K) = 0   (S - 1 = m / (27 K); e_j = 3 u_j - 1 = e0_j + 3 u0_j expm1(z_j)),
+//        r(0) >= 0 (AM-GM at P = 1/27) and r -> -inf as m -> 1; a root is a KKT point, so it is unique.  A safeguarded
+//        Newton in x = log(m / (1 - m)) finds it, with m and 1 - m both formed from x (no 1 - m cancellation at
+//        either end), dr/dm by the implicit derivative of E1: dtau/dm = (n_T l' + 1 / (1 - m)) / sum_T kap_j,
+//        dz_j/dm = l' - kap_j dtau/dm, kap_j = 1 + 1 / expm1(.)_j.
+// So 1 - K0 = m, S - 1 = sum e / 3 and the price-ratio denominators are never formed as differences near the peg.
+// Hessian.  On the traded set T, p_T = mu g(u), g = dPhi/du, and Phi(u) = 0: with Z a basis of g-perp on T,
+// du/dp = Z (Z'HZ)^-1 Z' / mu, H = d2Phi/du2 = a(w1' + 1w') + b ww' - Q diag(w^2), w = 1/u, a = 27 P K',
+// b = Q + 729 P^2 (S - 1) K''; since Z'w = -(K/Q) Z'1, Z'HZ = c (Z'1)(Z'1)' - Q Z'diag(w^2)Z with
+// c = (K/Q)(K - 2a + 729 P^2 (S - 1) K'' K / Q), and Z'1 = g_b - g_a = Q (u_a - u_b) / (u_a u_b) from e_a - e_b.
+// The scaled block Hs_ij = -p_i p_j (du/dp)_ij is PSD with Hs 1 = 0 (Z'p = 0), so it is the three edge weights
+// w_ij = -Hs_ij, (w01, w02, w12), 0 on an edge with an untraded end.  Writes D, L (flows) and w, returns the traded slots.
+// Fixed iteration caps, 3-element register arrays under full unrolling; shared by the per-thread solver and
+// k_eval_crypto3 (cfmm_kernels.cu).
+
+// E1 at s = log tau and dE1/ds; z and kap (0 off the traded set) out
+CFMM_HD inline double crypto3_e1(double s, const double* dB, double lg, const double* lu0, double l, double tgt,
+                                 double* z, double* kap, double& de, double& sc) {
+    const double tau = exp(s);
+    double f = -tgt, sk = 0.0;
+    sc = 1.0 + fabs(l) + fabs(tgt);
+CFMM_UNROLL
+    for (int j = 0; j < 3; ++j) {
+        const double eA = expm1(dB[j] + tau), eB = expm1(dB[j] + lg + tau);
+        const double bA = lu0[j] + log(eA);
+        const double zA = l - bA;
+        const double zB = eB > 0.0 ? l - (lu0[j] + log(eB)) : INFINITY;
+        z[j] = fmax(zA, 0.0) + fmin(zB, 0.0);
+        kap[j] = z[j] > 0.0 ? 1.0 + 1.0 / eA : (z[j] < 0.0 ? 1.0 + 1.0 / eB : 0.0);
+        f += z[j];
+        sk += kap[j];
+        sc += fabs(bA) + fabs(z[j]);
+    }
+    de = -tau * sk;
+    return f;
+}
+
+// the root of E1 in s = log tau, from s0 (bracketing, then a safeguarded Newton as stableswap_dir); z, kap out
+CFMM_HD inline double crypto3_tau(double s0, const double* dB, double lg, const double* lu0, double l, double tgt,
+                                  double* z, double* kap) {
+    constexpr double SMIN = -700.0, SMAX = 6.39;                        // tau in (1e-304, 600): exp, expm1 finite
+    double de = 0.0, sc = 0.0;
+    double s = fmin(fmax(s0, SMIN), SMAX), lo = s, hi = s;
+    if (crypto3_e1(s, dB, lg, lu0, l, tgt, z, kap, de, sc) > 0.0) {    // E1 falls in s
+        for (double step = 0.5; step <= 1024.0 && lo < SMAX; step *= 2.0) {
+            hi = fmin(lo + step, SMAX);
+            if (!(crypto3_e1(hi, dB, lg, lu0, l, tgt, z, kap, de, sc) > 0.0)) break;
+            lo = hi;
+        }
+    } else {
+        for (double step = 0.5; step <= 1024.0 && hi > SMIN; step *= 2.0) {
+            lo = fmax(hi - step, SMIN);
+            if (crypto3_e1(lo, dB, lg, lu0, l, tgt, z, kap, de, sc) > 0.0) break;
+            hi = lo;
+        }
+    }
+    double t = 0.5 * (lo + hi), dx_old = hi - lo, dx = dx_old;
+    for (int it = 0; it < 100; ++it) {
+        const double f = crypto3_e1(t, dB, lg, lu0, l, tgt, z, kap, de, sc);
+        if (f > 0.0) lo = t; else hi = t;
+        if (f == 0.0 || !(hi - lo > 4e-16 * (1.0 + fabs(t)))) break;
+        const double tn = t - f / de;
+        if (fabs(f) <= 4.5e-16 * sc) {                                  // E1 at the level of its own rounding
+            if (tn > lo && tn < hi) t = tn;
+            break;
+        }
+        if (!(tn > lo && tn < hi) || fabs(2.0 * f) > fabs(dx_old * de)) {
+            dx_old = dx; dx = 0.5 * (hi - lo); t = lo + dx;
+        } else {
+            dx_old = dx; dx = tn - t; t = tn;
+        }
+        if (fabs(dx) <= 1e-15 * (1.0 + fabs(t))) break;
+    }
+    crypto3_e1(t, dB, lg, lu0, l, tgt, z, kap, de, sc);
+    return t;
+}
+
+// r at x = log(m / (1 - m)) and dr/dx; the inner root s (warm start in, root out), z, kap, m, 1 - m, K, Q out
+CFMM_HD inline double crypto3_r(double x, double G, double ag2, const double* dB, double lg, const double* u0,
+                                const double* lu0, const double* e0, double sl0, double& s, double* z, double* kap,
+                                double& m, double& om, double& K, double& Q, double& dr, double& sc) {
+    m = 1.0 / (1.0 + exp(-x));
+    om = 1.0 / (1.0 + exp(x));
+    const double g = G + m;
+    K = ag2 * om / (g * g);
+    const double K1 = ag2 * (G + 1.0 + om) / (g * g * g);               // dK/dK0 = -dK/dm
+    const double qn = G + 3.0 * m - 2.0 * m * m;
+    Q = qn / (27.0 * g);
+    const double l = log(qn * g / (27.0 * ag2 * om));                   // log(Q / K)
+    const double tgt = log1p(-m) - sl0;
+    s = crypto3_tau(s, dB, lg, lu0, l, tgt, z, kap);
+    // dl/dm = Q'/Q + K'/K, Q' = 2 (G - 2 G m - m^2) / (27 (G + m)^2)
+    const double dl = 2.0 * (G - 2.0 * G * m - m * m) / (qn * g) + K1 / K;
+    int nt = 0;
+    double sk = 0.0;
+CFMM_UNROLL
+    for (int j = 0; j < 3; ++j) { nt += kap[j] != 0.0; sk += kap[j]; }
+    const double dtau = nt ? (nt * dl + 1.0 / om) / sk : 0.0;
+    double r = 0.0, d = 0.0;
+    sc = 1.0;
+CFMM_UNROLL
+    for (int j = 0; j < 3; ++j) {
+        const double ex = expm1(z[j]);
+        const double e = e0[j] + 3.0 * u0[j] * ex;
+        r += e;
+        sc += fabs(e0[j]) + fabs(3.0 * u0[j] * ex);
+        if (kap[j] != 0.0) d += 3.0 * u0[j] * (1.0 + ex) * (dl - kap[j] * dtau);
+    }
+    const double f = m * g * g / om;                                    // m / K = ag2 f
+    r -= f / (9.0 * ag2);
+    sc += f / (9.0 * ag2);
+    d -= (g * (G + 3.0 * m) / om + f / om) / (9.0 * ag2);
+    dr = d * m * om;
+    return r;
+}
+
+// The 2 x 2 (or 1 x 1) block -Hs on the traded set from the answer; see the header comment.  ia, ib, ic: the traded
+// slots (ic < 0: two traded).  Returns the edge weights in w[3] = (w01, w02, w12).
+CFMM_HD inline void crypto3_edges(int ia, int ib, int ic, const double* u, const double* e, const double* p, double mu,
+                                  double m, double om, double K, double Q, double K1, double K2, double* w) {
+    w[0] = w[1] = w[2] = 0.0;
+    const double Sm1 = m / (27.0 * K);
+    const double a = om * K1;
+    const double c = (K / Q) * (K - 2.0 * a + om * om * Sm1 * K2 * K / Q);
+    if (ic < 0) {                                                       // Z = (g_b, -g_a): 1 x 1
+        const double ga = K + Q / u[ia], gb = K + Q / u[ib];
+        const double wa = 1.0 / u[ia], wb = 1.0 / u[ib];
+        const double eta = Q * (e[ia] - e[ib]) / (3.0 * u[ia] * u[ib]);   // g_b - g_a
+        const double B = c * eta * eta - Q * (gb * gb * wa * wa + ga * ga * wb * wb);
+        if (B < 0.0) w[ia + ib - 1] = -p[ia] * p[ib] * ga * gb / (mu * B);   // edge (0,1) 0, (0,2) 1, (1,2) 2
+        return;
+    }
+    // three traded: Z = [(g1, -g0, 0), (g2, 0, -g0)] in slot order
+    const double g0 = K + Q / u[0], g1 = K + Q / u[1], g2 = K + Q / u[2];
+    const double w0 = 1.0 / u[0], w1 = 1.0 / u[1], w2 = 1.0 / u[2];
+    const double h1 = Q * (e[0] - e[1]) / (3.0 * u[0] * u[1]), h2 = Q * (e[0] - e[2]) / (3.0 * u[0] * u[2]);
+    const double b11 = c * h1 * h1 - Q * (g1 * g1 * w0 * w0 + g0 * g0 * w1 * w1);
+    const double b12 = c * h1 * h2 - Q * (g1 * g2 * w0 * w0);
+    const double b22 = c * h2 * h2 - Q * (g2 * g2 * w0 * w0 + g0 * g0 * w2 * w2);
+    const double det = b11 * b22 - b12 * b12;
+    if (!(det > 0.0) || !(b11 < 0.0)) return;
+    const double i11 = b22 / det, i12 = -b12 / det, i22 = b11 / det;
+    const double N01 = -g0 * (g1 * i11 + g2 * i12), N02 = -g0 * (g1 * i12 + g2 * i22), N12 = g0 * g0 * i12;
+    w[0] = p[0] * p[1] * N01 / mu;
+    w[1] = p[0] * p[2] * N02 / mu;
+    w[2] = p[1] * p[2] * N12 / mu;
+}
+
+// c_j = p_j / D; A, G: the whitepaper amplification and curve gamma.  Flows into D[3], L[3], edge weights into w[3];
+// returns the traded slots as a bit mask.
+CFMM_HD inline uint32_t cryptoswap3(double R0, double R1, double R2, double c0, double c1, double c2, double A,
+                                    double G, double gam, double n0, double n1, double n2, double* D, double* L,
+                                    double* w) {
+    const double R[3] = {R0, R1, R2}, cc[3] = {c0, c1, c2}, nu[3] = {n0, n1, n2};
+    double u0[3], lu0[3], e0[3], pi[3], dB[3], z[3], kap[3];
+    double pmin = INFINITY, sl0 = 0.0;
+CFMM_UNROLL
+    for (int j = 0; j < 3; ++j) {
+        D[j] = L[j] = w[j] = 0.0;
+        u0[j] = cc[j] * R[j];
+        lu0[j] = log(u0[j]);
+        e0[j] = fma(3.0, u0[j], -1.0);
+        sl0 += log1p(e0[j]);
+        pi[j] = nu[j] / cc[j];
+        pmin = fmin(pmin, pi[j]);
+    }
+    const double ag2 = A * G * G, lg = log(gam);
+    // the current point: m0 = 1 - 27 P0, K0 and Q0 on the curve, then the band
+    const double m0 = fmax(-expm1(sl0), 0.0), om0 = exp(sl0);
+    const double gq = G + m0;
+    const double Kc = ag2 * om0 / (gq * gq), Qc = (G + 3.0 * m0 - 2.0 * m0 * m0) / (27.0 * gq);
+    double cmax = -INFINITY, cmin = INFINITY;
+CFMM_UNROLL
+    for (int j = 0; j < 3; ++j) {
+        dB[j] = log(pi[j] / pmin);
+        const double cj = dB[j] - log(Kc + Qc / u0[j]);
+        cmax = fmax(cmax, cj);
+        cmin = fmin(cmin, cj);
+    }
+    if (!(lg + cmax > cmin)) return 0u;                                 // the no-trade band: exactly nothing
+    // outer: r(x) = 0 in x = logit(m), bracketed from the current m0
+    constexpr double XMAX = 700.0;
+    double s = 0.0, m = 0.0, om = 1.0, K = 0.0, Q = 0.0, dr = 0.0, sc = 0.0;
+    const double x0 = fmin(fmax(log(fmax(m0, 1e-300)) - log(om0), -XMAX), XMAX);
+    double lo = x0, hi = x0;
+    if (crypto3_r(x0, G, ag2, dB, lg, u0, lu0, e0, sl0, s, z, kap, m, om, K, Q, dr, sc) > 0.0) {   // r falls in x
+        for (double step = 1.0; step <= 1024.0 && lo < XMAX; step *= 2.0) {
+            hi = fmin(lo + step, XMAX);
+            if (!(crypto3_r(hi, G, ag2, dB, lg, u0, lu0, e0, sl0, s, z, kap, m, om, K, Q, dr, sc) > 0.0)) break;
+            lo = hi;
+        }
+    } else {
+        for (double step = 1.0; step <= 1024.0 && hi > -XMAX; step *= 2.0) {
+            lo = fmax(hi - step, -XMAX);
+            if (crypto3_r(lo, G, ag2, dB, lg, u0, lu0, e0, sl0, s, z, kap, m, om, K, Q, dr, sc) > 0.0) break;
+            hi = lo;
+        }
+    }
+    double t = 0.5 * (lo + hi), dx_old = hi - lo, dx = dx_old;
+    for (int it = 0; it < 100; ++it) {
+        const double f = crypto3_r(t, G, ag2, dB, lg, u0, lu0, e0, sl0, s, z, kap, m, om, K, Q, dr, sc);
+        if (f > 0.0) lo = t; else hi = t;
+        if (f == 0.0 || !(hi - lo > 4e-16 * (1.0 + fabs(t)))) break;
+        const double tn = t - f / dr;
+        if (fabs(f) <= 4.5e-16 * sc) {
+            if (tn > lo && tn < hi) t = tn;
+            break;
+        }
+        if (!(tn > lo && tn < hi) || fabs(2.0 * f) > fabs(dx_old * dr)) {
+            dx_old = dx; dx = 0.5 * (hi - lo); t = lo + dx;
+        } else {
+            dx_old = dx; dx = tn - t; t = tn;
+        }
+        if (fabs(dx) <= 1e-15 * (1.0 + fabs(t))) break;
+    }
+    crypto3_r(t, G, ag2, dB, lg, u0, lu0, e0, sl0, s, z, kap, m, om, K, Q, dr, sc);
+    // flows and the Hessian at the answer
+    const double g = G + m;
+    const double K1 = ag2 * (G + 1.0 + om) / (g * g * g), K2 = ag2 * (4.0 * G + 4.0 + 2.0 * om) / (g * g * g * g);
+    const double mu = pmin * exp(-exp(s)) / (gam * K);
+    double u[3], e[3], p[3];
+    uint32_t mask = 0u;
+    int ia = -1, ib = -1, ic = -1;
+CFMM_UNROLL
+    for (int j = 0; j < 3; ++j) {
+        const double ex = expm1(z[j]);
+        u[j] = u0[j] * exp(z[j]);
+        e[j] = e0[j] + 3.0 * u0[j] * ex;
+        p[j] = z[j] > 0.0 ? pi[j] / gam : pi[j];
+        if (z[j] != 0.0) {
+            if (z[j] > 0.0) D[j] = R[j] * ex / gam; else L[j] = -R[j] * ex;
+            mask |= 1u << j;
+            if (ia < 0) ia = j; else if (ib < 0) ib = j; else ic = j;
+        }
+    }
+    if (ib >= 0) crypto3_edges(ia, ib, ic, u, e, p, mu, m, om, K, Q, K1, K2, w);
+    return mask;
+}
+
 // n-coin StableSwap (Curve) pool, n = k = 2..KM coins.  Scaled balances y_j = r_j x_j, whitepaper amplification A,
 // a = A n^n, and D = D(R) the invariant of the current reserves (precomputed).  In units of D (u_j = y_j / D) the pool
 // keeps G(u) = a sum(u) + 1 - a - Q(u) >= 0, Q(u) = 1 / (n^n prod u); G is strictly concave on u > 0 and
@@ -643,7 +897,11 @@ CFMM_UNROLL
 // CRYPTO (with all three): also two-coin cryptoswap pools (kind 8) through cryptoswap_pair, c_j = p_j / D in the pool's
 // two w slots and (A, G) in its two logrw slots; cfmm_batch_solve_cryptoswap runs this fifth instance.  The other
 // instances give problems with such pools status 3.
-template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false>
+// CRYPTO3 (with all four): also three-coin cryptoswap pools (kind 9) through cryptoswap3, c_j = p_j / D in the pool's
+// three w slots and (A, G) in its first two logrw slots, the Hessian block added from the three edge weights;
+// cfmm_batch_solve_tricrypto runs this sixth instance.  The other instances give problems with such pools status 3.
+template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
+          bool CRYPTO3 = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane,
                                const double* rec = nullptr) {
@@ -660,7 +918,20 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
         const int k = (int)(P.pool_ptr[i + 1] - off);
         const double gam = P.gamma[i];
         double D[KMAX], L[KMAX];
-        if (CRYPTO && P.kind[i] == 8) {                                   // c = p / D in w, (A, G) in logrw
+        if (CRYPTO3 && P.kind[i] == 9) {                                  // c = p / D in w, (A, G) in logrw
+            double w[3];
+            const uint32_t mask = cryptoswap3(P.R[off], P.R[off + 1], P.R[off + 2], P.w[off], P.w[off + 1], P.w[off + 2],
+                                              P.logrw[off], P.logrw[off + 1], gam, nu[P.tok[off]], nu[P.tok[off + 1]],
+                                              nu[P.tok[off + 2]], D, L, w);
+            if (Hs && mask) {                                              // Hs = sum_{a<b} w_ab (e_a - e_b)(e_a - e_b)'
+                for (int q = 0; q < 3; ++q) {
+                    if (w[q] == 0.0) continue;
+                    const int ta = P.tok[off + (q == 2 ? 1 : 0)], tb = P.tok[off + (q == 0 ? 1 : 2)];
+                    (*Hs)[ta * n + ta] += w[q]; (*Hs)[tb * n + tb] += w[q];
+                    (*Hs)[ta * n + tb] -= w[q]; (*Hs)[tb * n + ta] -= w[q];
+                }
+            }
+        } else if (CRYPTO && P.kind[i] == 8) {                            // c = p / D in w, (A, G) in logrw
             double hc = 0.0;
             cryptoswap_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], P.logrw[off], P.logrw[off + 1], gam,
                             nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
@@ -897,7 +1168,8 @@ CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL 
 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
 // rec: the concentrated pools' records (LADDER instance only).
-template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false>
+template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
+          bool CRYPTO3 = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0, const double* rec = nullptr) {
     const int n = Q.n;
@@ -917,9 +1189,10 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int64_t o = P.pool_ptr[i];
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1;
-        bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6) && !(CRYPTO && P.kind[i] == 8)) || k < 2 ||
+        bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6) && !(CRYPTO && P.kind[i] == 8) &&
+               !(CRYPTO3 && P.kind[i] == 9)) || k < 2 ||
               k > KMAX || ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
-                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8)) && k != 2);
+                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8)) && k != 2) || (CRYPTO3 && P.kind[i] == 9 && k != 3);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
     if (bad) {
@@ -946,7 +1219,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -992,7 +1265,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -1017,8 +1290,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -1043,8 +1316,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

@@ -479,3 +479,61 @@ def synth_crypto_market(m, n_tokens, seed, frac_crypto=0.4, far=0.5, mispricing=
                    np.concatenate([base.lad_sc, np.zeros((n_cs, 2))]), cg)
     assert hp.m == m0 + n_cs
     return hp, p
+
+
+TRICRYPTO_A_MULTIPLIER = 10000      # tricrypto-ng stores A() = A * N^N * A_MULTIPLIER (N = 3), gamma() as 1e18 fixed point
+
+
+def tricrypto_pool(A_raw, gamma_raw, price_scale, precisions, balances, mid_fee, out_fee, fee_gamma):
+    """A three-coin Curve v2 (tricrypto-ng) pool's on-chain state as this package's three-token 'cryptoswap' pool.
+    A_raw = A(), gamma_raw = gamma() (1e18 fixed point), price_scale = (price_scale(0), price_scale(1)) (coins 1 and 2 in
+    coin 0, 1e18 fixed point), precisions = the contract's 10^(18 - decimals_j), balances = balances(0..2) (raw integers),
+    mid_fee / out_fee (1e10 fixed point) and fee_gamma (1e18).  Returns (weights, reserves, gamma): weights =
+    (A, G, p_0, p_1, p_2) for HostPools.from_lists, reserves in whole tokens (balance * precision / 1e18) and the fee
+    gamma = 1 - fee at the current state, fee = mid_fee f + out_fee (1 - f), f = fee_gamma / (fee_gamma + 1 - K0),
+    K0 = 27 y0 y1 y2 / (y0 + y1 + y2)^3 with y = p * reserves (the contract's fee is charged on the output and moves with
+    the trade, so this gamma is the pool's fee for small trades only, as for twocrypto_pool).  A = A_raw /
+    (A_MULTIPLIER * 3^3) and G = gamma_raw / 1e18: the convention of the contract's comments; it has not been checked
+    against the contract's integer newton_D (see INTEGRATION.md)."""
+    A = float(A_raw) / (TRICRYPTO_A_MULTIPLIER * 27)
+    G = float(gamma_raw) / 1e18
+    x = np.array([float(balances[j]) * float(precisions[j]) for j in range(3)]) / 1e18
+    p = np.array([1.0, float(price_scale[0]) / 1e18, float(price_scale[1]) / 1e18])
+    y = p * x
+    K0 = 27.0 * y[0] * y[1] * y[2] / y.sum() ** 3
+    fg = float(fee_gamma) / 1e18
+    f = fg / (fg + 1.0 - K0)
+    fee = (float(mid_fee) * f + float(out_fee) * (1.0 - f)) / 1e10
+    return (A, G, float(p[0]), float(p[1]), float(p[2])), tuple(float(v) for v in x), 1.0 - fee
+
+
+def synth_tricrypto_market(m, n_tokens, seed, frac_tri=0.3, far=0.5, mispricing=0.02, T=(1, 16)):
+    """A market of three-coin cryptoswap pools beside every other kind: a frac_tri share of m pools are tricrypto pools
+    on random token triples (A in {0.1 .. 50}, curve gamma in {1e-5 .. 2e-2}, fees 0.05 .. 0.45 %), value-balanced within
+    a few percent; the price scales of a `far` share of them sit 20 % .. 4x away from the market prices, the others within
+    0.5 %.  The rest is synth_crypto_market's mix (two-coin cryptoswap, constant product, StableSwap, constant sum,
+    ranges and ladders).  n_tokens >= 3.  Returns (HostPools, prices)."""
+    from .pools import HostPools, KIND_CRYPTOSWAP_HOST
+    rng = np.random.default_rng(seed + 104729)
+    n_t = int(round(frac_tri * m))
+    base, p = synth_crypto_market(m - n_t, n_tokens, seed, mispricing=mispricing, T=T)
+    tri = np.stack([rng.choice(n_tokens, 3, replace=False) for _ in range(n_t)]) if n_t else np.zeros((0, 3), int)
+    off = rng.random(n_t) < far
+    sh = np.where(off[:, None], np.exp(rng.choice([-1.0, 1.0], (n_t, 3)) * rng.uniform(np.log(1.2), np.log(4.0), (n_t, 3))),
+                  np.exp(rng.uniform(-0.005, 0.005, (n_t, 3))))
+    sh[:, 0] = 1.0
+    scales = p[tri] * sh                                         # the pool's internal prices are off by sh
+    V = np.exp(9.0 + 1.5 * rng.standard_normal(n_t))
+    R = V[:, None] / scales * np.exp(mispricing * rng.standard_normal((n_t, 3)))
+    A = np.array([0.1, 1.0, 6.3, 50.0])[rng.integers(0, 4, n_t)]
+    G = np.array([1e-5, 1.45e-4, 2e-3, 2e-2])[rng.integers(0, 4, n_t)]
+    gam = np.array([0.9995, 0.9974, 0.9955])[rng.integers(0, 3, n_t)]
+    hp = HostPools(n_tokens, np.concatenate([base.pool_ptr, base.pool_ptr[-1] + 3 * np.arange(1, n_t + 1)]).astype(np.int64),
+                   np.concatenate([base.tok_idx, tri.ravel()]).astype(np.int32),
+                   np.concatenate([base.reserves, R.ravel()]), np.concatenate([base.weights, scales.ravel()]),
+                   np.concatenate([base.gamma, gam]),
+                   np.concatenate([base.kind, np.full(n_t, KIND_CRYPTOSWAP_HOST, np.uint8)]).astype(np.uint8),
+                   np.concatenate([base.amp, A]), None,
+                   np.concatenate([base.lad_ptr, np.full(n_t, base.lad_ptr[-1], np.int64)]), base.lad_rec,
+                   np.concatenate([base.lad_sc, np.zeros((n_t, 2))]), np.concatenate([np.asarray(base.cgam, float), G]))
+    return hp, p

@@ -24,7 +24,7 @@ KIND_STABLESWAP_HOST = 4  # StableSwap (Curve), 2..8 coins; rates ride in `weigh
 ANN_MAX = 4e7           # largest StableSwap coefficient A n^n accepted, any coin count (A <= 1e7 for two coins)
 STABLE_ARITY_MAX = 8    # most coins of a StableSwap pool
 KIND_CONCENTRATED_HOST = 6  # concentrated liquidity: a whole Uniswap-v3 tick ladder; records in HostPools.lad_rec
-KIND_CRYPTOSWAP_HOST = 8  # two-coin Curve cryptoswap; price scales ride in `weights`, A in HostPools.amp, gamma in .cgam
+KIND_CRYPTOSWAP_HOST = 8  # Curve cryptoswap, 2 or 3 coins; price scales ride in `weights`, A in HostPools.amp, gamma in .cgam
 CRYPTO_A_RANGE = (1e-6, 1e4)       # accepted whitepaper A of cryptoswap pools (the concavity of D is checked over it)
 CRYPTO_GAMMA_RANGE = (1e-6, 0.1)   # accepted curve gamma of cryptoswap pools (tests/test_cryptoswap.py checks the corners)
 LADDER_T_MAX = 1 << 20  # most intervals of one concentrated pool (cfmm_small::LADDER_T_MAX)
@@ -304,10 +304,66 @@ def cryptoswap_invariant(reserves, scales, amp, cgam) -> np.ndarray:
     return out * scale
 
 
+def tricrypto_invariant(reserves, scales, amp, cgam) -> np.ndarray:
+    """Invariant D of three-coin cryptoswap pools (tricrypto-ng): with y = scales * reserves, S = sum y, P = prod y,
+    K0 = 27 P / D^3 and K = A K0 G^2 / (G + 1 - K0)^2 the root D in [3 P^(1/3), S] of
+        K D^2 S + P = K D^3 + (D/3)^3,   i.e.   F(D) = K (S - D) - (1 - K0) D / 27 = 0.
+    reserves, scales: (m, 3); amp: (m,), the whitepaper A; cgam: (m,), the curve gamma G.  Newton's method on F in D, in
+    fp64 and in units of S (homogeneous: nothing over- or underflows), from the upper bound D = S, kept inside the
+    bracket by a bisection step whenever Newton would leave it.  Where every |e_j| < 1, e_j = 3 y_j / D - 1, 1 - K0 is
+    formed as -(e_0 + e_1 + e_2 + e_0 e_1 + e_0 e_2 + e_1 e_2 + e_0 e_1 e_2) with e_0 + e_1 + e_2 = 3 (S - D) / D: no
+    cancellation near the peg; elsewhere as 1 - 27 P / D^3.  A pool stops once a step moves D by at most 2 ulp.  Elementwise, each pool's arithmetic in a fixed
+    order: a subset (PoolStore.update_pools) gives the same bits as the whole."""
+    y = np.asarray(reserves, np.float64).reshape(-1, 3) * np.asarray(scales, np.float64).reshape(-1, 3)
+    A = np.asarray(amp, np.float64).reshape(-1)
+    G = np.asarray(cgam, np.float64).reshape(-1)
+    scale = y.sum(1)
+    with np.errstate(all="ignore"):
+        u = y / scale[:, None]
+        S = u.sum(1)
+        lo, hi = 3.0 * np.cbrt(u[:, 0] * u[:, 1] * u[:, 2]), S.copy()
+        out = S.copy()
+        act = np.arange(len(S))
+        for _ in range(255):
+            if len(act) == 0:
+                break
+            d, a, g, s_ = out[act], A[act], G[act], S[act]
+            e = (3.0 * u[act] - d[:, None]) / d[:, None]
+            # near the peg (every |e_j| < 1) from the e_j; far from it 27 P / D^3 directly (the e_j terms cancel there)
+            near = np.abs(e).max(1) < 1.0
+            K0 = np.where(near, 0.0, 27.0 * (u[act, 0] / d) * (u[act, 1] / d) * (u[act, 2] / d))
+            m = np.where(near, -(3.0 * (s_ - d) / d + (e[:, 0] * e[:, 1] + e[:, 0] * e[:, 2] + e[:, 1] * e[:, 2])
+                                 + e[:, 0] * e[:, 1] * e[:, 2]), 1.0 - K0)
+            K0 = np.where(near, 1.0 - m, K0)
+            gm = g + m
+            K = a * K0 * g * g / (gm * gm)
+            K1 = a * g * g * (g + 1.0 + K0) / (gm * gm * gm)              # dK/dK0
+            f = K * (s_ - d) - m * d / 27.0
+            # dF/dD: dK0/dD = -3 K0 / D, dm/dD = 3 K0 / D
+            fp = -3.0 * K0 * K1 * (s_ - d) / d - K - (m + 3.0 * K0) / 27.0
+            lo[act] = np.where(f > 0, d, lo[act])
+            hi[act] = np.where(f > 0, hi[act], d)
+            dn = d - f / fp
+            dn = np.where(f == 0, d, np.where((dn > lo[act]) & (dn < hi[act]), dn, 0.5 * (lo[act] + hi[act])))
+            out[act] = dn
+            act = act[~((np.abs(dn - d) <= 4.5e-16 * dn) | (f == 0))]
+    return out * scale
+
+
+def cryptoswap_invariant_any(reserves, scales, amp, cgam) -> np.ndarray:
+    """cryptoswap_invariant or tricrypto_invariant by the pools' coin count (the last axis of reserves: 2 or 3)"""
+    n = np.asarray(reserves).shape[-1]
+    return (cryptoswap_invariant if n == 2 else tricrypto_invariant)(reserves, scales, amp, cgam)
+
+
 def _crypto_groups(kind, pool_ptr):
-    """(pool ids, (m, 2) CSR offsets) of the cryptoswap pools"""
+    """(n, pool ids, (m, n) CSR offsets) of the cryptoswap pools, one entry per coin count"""
     cs = np.nonzero(np.asarray(kind) == KIND_CRYPTOSWAP_HOST)[0]
-    return cs, np.asarray(pool_ptr, np.int64)[cs][:, None] + np.arange(2)
+    if len(cs) == 0:
+        return []
+    ptr = np.asarray(pool_ptr, np.int64)
+    ar = ptr[cs + 1] - ptr[cs]
+    return [(int(k), cs[ar == k], ptr[cs[ar == k]][:, None] + np.arange(k)) for k in np.unique(ar).tolist()]
 
 
 def _stable_groups(kind, pool_ptr):
@@ -358,9 +414,10 @@ class HostPools:
             self.inv = np.zeros(m)
             for _, ss, off in _stable_groups(self.kind, self.pool_ptr):
                 self.inv[ss] = stableswap_invariant_any(self.reserves[off], self.weights[off], self.amp[ss])
-            cs, off = _crypto_groups(self.kind, self.pool_ptr)
-            if len(cs):
-                self.inv[cs] = cryptoswap_invariant(self.reserves[off], self.weights[off], self.amp[cs], self.cgam[cs])
+            for k, cs, off in _crypto_groups(self.kind, self.pool_ptr):
+                if k in (2, 3):
+                    self.inv[cs] = cryptoswap_invariant_any(self.reserves[off], self.weights[off], self.amp[cs],
+                                                            self.cgam[cs])
 
     @property
     def m(self) -> int:
@@ -380,7 +437,9 @@ class HostPools:
         must be None: the real reserves are derived (ladder_state).  And 'cryptoswap' (a two-coin Curve v2 pool, twocrypto-ng):
         weights[i] = (A, G, p_0, p_1) with A the whitepaper amplification (K -> A K0 as G -> inf, StableSwap's A), G the
         curve's gamma (not the fee) and p_j the price scale times the precision of coin j (only p_0 / p_1 matters);
-        A in CRYPTO_A_RANGE, G in CRYPTO_GAMMA_RANGE.  instances.twocrypto_pool converts a contract's state."""
+        A in CRYPTO_A_RANGE, G in CRYPTO_GAMMA_RANGE.  instances.twocrypto_pool converts a contract's state.  Three
+        tokens (tricrypto-ng): weights[i] = (A, G, p_0, p_1, p_2), the same A and G rules, invariant tricrypto_invariant;
+        instances.tricrypto_pool converts a contract's state."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
@@ -429,8 +488,9 @@ class HostPools:
                 kd.append(KIND_STABLESWAP_HOST); wts += [float(x) for x in p[1:]]; amp[i] = p[0]
             elif kinds[i] == "cryptoswap":
                 p = None if (weights is None or weights[i] is None) else np.asarray(weights[i], float).reshape(-1)
-                if k != 2 or p is None or len(p) != 4:
-                    raise ValueError(f"pool {i}: cryptoswap needs 2 tokens and weights[i] = (A, gamma, p_0, p_1)")
+                if k not in (2, 3) or p is None or len(p) != k + 2:
+                    raise ValueError(f"pool {i}: cryptoswap needs 2 or 3 tokens and weights[i] = (A, gamma, p_0, ..., "
+                                     "p_{n-1})")
                 _check_cryptoswap(p[0], p[1], p[2:], reserves[i], f"pool {i}: ")
                 kd.append(KIND_CRYPTOSWAP_HOST); wts += [float(x) for x in p[2:]]; amp[i] = p[0]; cgam[i] = p[1]
             elif kinds[i] in ("geomean", "product"):
@@ -501,10 +561,9 @@ class HostPools:
             D = np.asarray(self.inv, float)[ss]
             if not bool(np.all(np.isfinite(D) & (D > 0))):
                 raise ValueError("stableswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
-        cs, off = _crypto_groups(self.kind, self.pool_ptr)
-        if len(cs):
-            if np.any(np.diff(self.pool_ptr)[cs] != 2):
-                raise ValueError("cryptoswap pools must have 2 tokens")
+        for k, cs, off in _crypto_groups(self.kind, self.pool_ptr):
+            if k not in (2, 3):
+                raise ValueError("cryptoswap pools must have 2 or 3 tokens")
             _check_cryptoswap(self.amp[cs], np.asarray(self.cgam, float)[cs], self.weights[off], self.reserves[off])
             D = np.asarray(self.inv, float)[cs]
             if not bool(np.all(np.isfinite(D) & (D > 0))):
@@ -618,7 +677,7 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
     pool pool_ids[k], the triple of HostPools.from_lists' weights[i] (T may differ from the pool's old T; the rules of
     from_lists); not together with prices=.  amp[k]: the new whitepaper A of StableSwap pool pool_ids[k], rates[k]: its new
     rate vector (the pool's arity; an (n, k) array as for reserves), under the rules of from_lists.  For cryptoswap pools
-    amp[k] is the new whitepaper A, rates[k] the new price scales (p_0, p_1), curve_gamma[k] the new curve gamma (cryptoswap
+    amp[k] is the new whitepaper A, rates[k] the new price scales (p_0, p_1[, p_2]), curve_gamma[k] the new curve gamma (cryptoswap
     pools only); amp= and rates= may not mix StableSwap and cryptoswap pools in one call.
     Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order."""
     m = len(pool_ptr) - 1
@@ -704,7 +763,7 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             W = _pool_rows(rates, n, ar, "rates")
         _check_cryptoswap(np.full(n, CRYPTO_A_RANGE[0]) if A is None else A,
                           np.full(n, CRYPTO_GAMMA_RANGE[0]) if CG is None else CG,
-                          np.ones((n, 2)) if W is None else W.reshape(n, 2), np.ones((n, 2)))
+                          np.ones(n) if W is None else W, np.ones(n))
     elif amp is not None or rates is not None:
         if not bool(np.all(np.asarray(kind)[ids] == KIND_STABLESWAP_HOST)):
             raise ValueError("amp= and rates= apply to StableSwap or cryptoswap pools only (not both in one call)")
@@ -805,9 +864,12 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         keys.append((_lib.KIND_CONCENTRATED, 2, np.nonzero(cl)[0]))
     cs = hp.kind == KIND_CRYPTOSWAP_HOST
     if cs.any():
-        if np.any(ar[cs] != 2):
-            raise ValueError("cryptoswap pools must have 2 tokens")
-        keys.append((_lib.KIND_CRYPTOSWAP, 2, np.nonzero(cs)[0]))
+        if np.any((ar[cs] != 2) & (ar[cs] != 3)):
+            raise ValueError("cryptoswap pools must have 2 or 3 tokens")
+        if np.any(cs & (ar == 2)):                  # two coins: the kind-8 bucket (k_eval_crypto)
+            keys.append((_lib.KIND_CRYPTOSWAP, 2, np.nonzero(cs & (ar == 2))[0]))
+        if np.any(cs & (ar == 3)):                  # three: the kind-9 bucket (k_eval_crypto3)
+            keys.append((_lib.KIND_CRYPTOSWAP_3, 3, np.nonzero(cs & (ar == 3))[0]))
     gm = (hp.kind == KIND_GEOMEAN_HOST) & ~is_cp
     for k in np.unique(ar[gm]).tolist():
         if k < 2 or k > 32:
@@ -866,7 +928,7 @@ class DeviceBucket:
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
             AD = np.stack([hp.amp[spec.sel], hp.inv[spec.sel]])
             self.logrw = torch.as_tensor(_padded(AD, self.stride, 1.0), **f64)
-        if self.kind == _lib.KIND_CRYPTOSWAP:              # price scales in the weights slot, (A, G, D) in three logrw rows
+        if self.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3):   # price scales in weights, (A, G, D) in logrw
             self.weights = torch.as_tensor(_padded(hp.weights[spec.off], self.stride, 1.0), **f64)
             AGD = np.stack([hp.amp[spec.sel], np.asarray(hp.cgam, np.float64)[spec.sel], hp.inv[spec.sel]])
             self.logrw = torch.as_tensor(_padded(AGD, self.stride, 1.0), **f64)
@@ -920,9 +982,9 @@ class DeviceBucket:
             if self.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N):
                 if AD is None:
                     self.logrw[1, li] = torch.as_tensor(stableswap_invariant_any(R.T, W.T, amp), **f64)
-            elif self.kind == _lib.KIND_CRYPTOSWAP:
+            elif self.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3):
                 if AD is None:
-                    self.logrw[2, li] = torch.as_tensor(cryptoswap_invariant(R.T, W.T, amp, cgam), **f64)
+                    self.logrw[2, li] = torch.as_tensor(cryptoswap_invariant_any(R.T, W.T, amp, cgam), **f64)
             elif self.kind == _lib.KIND_GEOMEAN:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
         if rates is not None:
@@ -978,7 +1040,8 @@ class DeviceBucket:
             self.lam = torch.zeros((self.arity, self.stride), **f64)
         if hess and self.hcoef is None:
             # n-coin StableSwap: one coefficient h_j per slot ([arity][stride]); every other kind: one per pool
-            self.hcoef = torch.zeros((self.arity, self.stride) if self.kind == _lib.KIND_STABLESWAP_N else self.stride,
+            self.hcoef = torch.zeros((self.arity, self.stride)
+                                     if self.kind in (_lib.KIND_STABLESWAP_N, _lib.KIND_CRYPTOSWAP_3) else self.stride,
                                      **f64)
             self.hmask = torch.zeros(self.stride, dtype=torch.int32, device=self._device)
         return _lib.EvalOut(self.delta.data_ptr() if trades else None, self.lam.data_ptr() if trades else None,
@@ -1478,6 +1541,7 @@ class PoolStore:
                         else 80 if b.kind == _lib.KIND_CONCENTRATED
                         else 64 if b.kind == _lib.KIND_STABLESWAP
                         else 72 if b.kind == _lib.KIND_CRYPTOSWAP
+                        else 148 if b.kind == _lib.KIND_CRYPTOSWAP_3
                         else 20 * b.arity + 24 if b.kind == _lib.KIND_STABLESWAP_N else 32)
         return n + 16 * self.n_tokens + 8
 
@@ -1655,9 +1719,9 @@ class PoolStore:
                 A = u.amp[e] if u.amp is not None else self._amp_host[ids]
                 rt = u.rates[rs] if u.rates is not None else self._weights_host[u.slots[rs]]
                 Rd = R if R is not None else b.reserves[:, torch.as_tensor(loc[ids], device=self.device)].cpu().numpy()
-                if b.kind == _lib.KIND_CRYPTOSWAP:
+                if b.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3):
                     G = u.curve_gamma[e] if u.curve_gamma is not None else self._cgam_host[ids]
-                    D = cryptoswap_invariant(Rd.T, rt.T, A, G)
+                    D = cryptoswap_invariant_any(Rd.T, rt.T, A, G)
                     AD = np.stack([A, G, D])
                 else:
                     D = stableswap_invariant_any(Rd.T, rt.T, A)
@@ -1676,9 +1740,9 @@ class PoolStore:
             if lad is not None:
                 b.splice_ladders(self.lib, l, lad[0], lad[1], lad[2], lad[3], self._stream())
             W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None and AD is None) else None
-            amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N,
-                                                     _lib.KIND_CRYPTOSWAP) else None
-            cg_ = self._cgam_host[ids] if b.kind == _lib.KIND_CRYPTOSWAP else None
+            crypto = b.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3)
+            amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) or crypto else None
+            cg_ = self._cgam_host[ids] if crypto else None
             b.write_update(l, R, g, W, amp_, sc, None if u.rates is None else rt, AD, cg_)
         # the store's host state, once the device holds the update
         for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:
@@ -1690,7 +1754,7 @@ class PoolStore:
                     self._cgam_host = self._cgam_host.copy()
                     self._own_stable = True
                 self._amp_host[ids] = AD[0]
-                if b.kind == _lib.KIND_CRYPTOSWAP:
+                if b.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3):
                     self._cgam_host[ids] = AD[1]
                 self._weights_host[u.slots[rs]] = rt
         torch.cuda.synchronize(self.device)

@@ -67,7 +67,17 @@ enum {
                               whitepaper amplification: K -> A K0 as G -> inf, StableSwap's A), slot 1 = G (the curve's
                               gamma, not the fee), slot 2 = D of the current reserves.  hcoef is per pool, as for every
                               pair kind.  Smooth: no theta_bar.  (7 is not a kind: cfmm_arb_eval returns CFMM_E_KIND
-                              for it, as for any other unknown kind.)                                                 */
+                              for it, as for any other unknown kind.)                                                 */,
+    CFMM_KIND_CRYPTOSWAP_3 = 9 /* three-coin Curve cryptoswap (tricrypto-ng): y_j = p_j x_j, K0 = 27 y0 y1 y2 / D^3,
+                              K = A K0 G^2 / (G + 1 - K0)^2, and the pool keeps D(y) >= D(R) for the root D of
+                              K D^2 (y0 + y1 + y2) + y0 y1 y2 = K D^3 + (D/3)^3 with 3 (y0 y1 y2)^(1/3) <= D <=
+                              y0 + y1 + y2.  Not in the reference; arity 3 (any other arity: CFMM_E_KIND).
+                              weights [3][stride] = the price scales (p0, p1, p2) > 0; logrw [3][stride]: slot 0 = A,
+                              slot 1 = G, slot 2 = D of the current reserves, as for kind 8.  hcoef is [3][stride]: the
+                              edge weights (w01, w02, w12) of the pool's scaled Hessian block, Hs = sum_{a<b} w_ab
+                              (e_a - e_b)(e_a - e_b)' (Hs 1 = 0; one weight may be negative, Hs is PSD), 0 on an edge
+                              with an untraded end; hmask = the traded slots (required by the HVP, diagonal and dense
+                              kernels).  Smooth: no theta_bar                                                        */
 };
 
 enum {
@@ -328,15 +338,18 @@ typedef struct cfmm_csr_pools {
     const double* weights;     /* [nnz]  normalised like cp.geo_mean(p=...), arbitrage.py:65; 0 on constant-sum pools;
                                          offsets of bounded products; rates of StableSwap pools; concentrated
                                          pools: the sqrt price s at the first slot, c at the second;
-                                         cryptoswap pools: p_j / D, the price scales over the invariant
-                                         of the reserves (u = weights * reserves in units of D)         */
+                                         cryptoswap pools (kinds 8, 9): p_j / D, the price scales over
+                                         the invariant of the reserves (u = weights * reserves in units
+                                         of D)                                                          */
     const double* logrw;       /* [nnz]  log(reserves / weights) (unused on constant-sum pools); StableSwap: A at the
                                          pool's first slot, D at its second; concentrated pools: the index of
                                          the first record at the first slot, T at the second; cryptoswap
-                                         pools: A at the first slot, the curve gamma G at the second    */
+                                         pools (kinds 8, 9): A at the first slot, the curve gamma G at
+                                         the second                                                     */
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
     const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP |
-                                            CFMM_KIND_CONCENTRATED | CFMM_KIND_CRYPTOSWAP, else weighted
+                                            CFMM_KIND_CONCENTRATED | CFMM_KIND_CRYPTOSWAP |
+                                            CFMM_KIND_CRYPTOSWAP_3, else weighted
                                             geometric mean                                           */
 } cfmm_csr_pools;
 
@@ -391,6 +404,12 @@ int cfmm_batch_solve_concentrated(const cfmm_csr_pools* pools, const double* rec
  * concentrated pools.  A fifth kernel instance, so the others keep their registers.  Same limits and workspace. */
 int cfmm_batch_solve_cryptoswap(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
                                 const cfmm_batch_params* prm, void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_CRYPTOSWAP_3 pools (three coins; p_j / D in the three weights slots,
+ * (A, G) in the first two logrw slots), beside every kind cfmm_batch_solve_cryptoswap takes (the five entry points
+ * above give their problems status 3).  records: as for cfmm_batch_solve_cryptoswap.  A sixth kernel instance, so the
+ * others keep their registers.  Same limits and workspace. */
+int cfmm_batch_solve_tricrypto(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
+                               const cfmm_batch_params* prm, void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
