@@ -46,6 +46,12 @@ class SolveParams(C.Structure):
     _fields_ = [("tol", C.c_double), ("nu_floor", C.c_double), ("max_iter", C.c_int32), ("cg_max", C.c_int32)]
 
 
+class MarketParams(C.Structure):
+    _fields_ = [("tol", C.c_double), ("nu_floor", C.c_double), ("eps0", C.c_double), ("eps_min", C.c_double),
+                ("eps_shrink", C.c_double), ("max_iter", C.c_int32), ("cg_max", C.c_int32), ("max_outer", C.c_int32),
+                ("linear_solver", C.c_int32)]
+
+
 class SolveResult(C.Structure):
     _fields_ = [("dual_value", C.c_double), ("primal_value", C.c_double), ("gap", C.c_double),
                 ("primal_infeas", C.c_double), ("err", C.c_double), ("iters", C.c_int32), ("evals", C.c_int32),
@@ -143,6 +149,14 @@ def load(build_if_missing: bool = True):
     lib.cfmm_blocked_solve_peer.argtypes = [C.POINTER(BlockedPairs), i32, vp, vp, vp, vp, vp, vp, vp,
                                             C.POINTER(SolveParams), C.POINTER(SolveResult), C.POINTER(PeerCtx), vp]
     lib.cfmm_blocked_solve_peer.restype = C.c_int
+    lib.cfmm_market_solve_work_bytes.argtypes = [C.POINTER(Bucket), i32, C.POINTER(BlockedPairs), i32, i32]
+    lib.cfmm_market_solve_work_bytes.restype = i64
+    lib.cfmm_market_solve.argtypes = [C.POINTER(Bucket), C.POINTER(EvalOut), i32, C.POINTER(BlockedPairs),
+                                      C.POINTER(EvalOut), i32, vp, vp, vp, vp, vp, vp, vp, C.POINTER(MarketParams),
+                                      C.POINTER(SolveResult), vp]
+    lib.cfmm_market_solve.restype = C.c_int
+    lib.cfmm_dense_cholesky.argtypes = [i32, vp, vp, vp]
+    lib.cfmm_dense_cholesky.restype = C.c_int
     lib.cfmm_persist_solve_work_bytes.argtypes = [C.POINTER(BlockedPairs), i32]
     lib.cfmm_persist_solve_work_bytes.restype = i64
     lib.cfmm_persist_solve.argtypes = lib.cfmm_blocked_solve_peer.argtypes

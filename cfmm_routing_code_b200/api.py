@@ -233,6 +233,57 @@ def _solve_native(store: PoolStore, spec, nu0, tol, max_iter, cg_max=200, impl="
                      hvps=res.hvps, status=status, wall_s=time.perf_counter() - t0, history=[])
 
 
+MARKET_KW = ("linear_solver", "cg_max", "eps", "eps_min", "eps_shrink", "max_outer")
+
+
+def _market_applicable(store: PoolStore, native, verbose, solver_kw) -> bool:
+    """native="hostloop" on a single-GPU store of any pool kinds, with solver.py keywords the C++ loop takes"""
+    return native == "hostloop" and store.world == 1 and not verbose and all(k in MARKET_KW for k in solver_kw)
+
+
+def _solve_market(store: PoolStore, spec, nu0, tol, max_iter, linear_solver="auto", cg_max=200, eps=0.1,
+                  eps_min=1e-4, eps_shrink=0.5, max_outer=60) -> SolveInfo:
+    """The whole of solver.py's loop in one C call (cfmm_market_solve, csrc/cfmm_solver.cu): every pool kind, the dense or
+    PCG Newton systems and the method of multipliers, with the final read-back's trades left in the store's buckets."""
+    import ctypes as C
+    import time
+    from .solver import default_nu0
+    t0 = time.perf_counter()
+    ls = {"auto": 0, "dense": 1, "cg": 2}.get(linear_solver)
+    if ls is None:
+        raise ValueError("linear_solver must be 'auto', 'dense' or 'cg'")
+    n, dev = store.n_tokens, store.device
+    f64 = dict(dtype=torch.float64, device=dev)
+    c = torch.as_tensor(np.asarray(spec.c, float), **f64)
+    a = torch.as_tensor(np.asarray(spec.a, float), **f64)
+    eq = torch.as_tensor(np.asarray(spec.eq, np.uint8), device=dev)
+    pinned = torch.as_tensor(np.asarray(spec.pinned, np.uint8), device=dev)
+    nu = torch.as_tensor(default_nu0(spec) if nu0 is None else np.asarray(nu0, float), **f64).clone()
+    psi = torch.empty(n, **f64)
+    buckets, outs, nb, blk, blk_out = store.market_structs()
+    blk_p = C.byref(blk) if blk is not None else None
+    nbytes = store.lib.cfmm_market_solve_work_bytes(buckets, nb, blk_p, n, ls)
+    _lib.check(min(int(nbytes), 0), "cfmm_market_solve_work_bytes")
+    if getattr(store, "_market_work", None) is None or store._market_work.numel() < nbytes:
+        store._market_work = None
+        store._market_work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    scale = max(float(np.abs(spec.c).max()), 1.0)
+    prm = _lib.MarketParams(float(tol), 1e-12 * scale, float(eps), float(eps_min), float(eps_shrink), int(max_iter),
+                            int(cg_max), int(max_outer), ls)
+    res = _lib.SolveResult()
+    st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    rc = store.lib.cfmm_market_solve(buckets, outs, nb, blk_p, C.byref(blk_out) if blk_out is not None else None, n,
+                                     c.data_ptr(), a.data_ptr(), eq.data_ptr(), pinned.data_ptr(), nu.data_ptr(),
+                                     psi.data_ptr(), store._market_work.data_ptr(), C.byref(prm), C.byref(res), st)
+    _lib.check(rc, "cfmm_market_solve")
+    store.evals += res.evals
+    store.hvps += res.hvps
+    status = {0: "optimal", 1: "max_iter", 2: "stalled"}[res.status]
+    return SolveInfo(nu=nu, psi=psi, dual_value=res.dual_value, primal_value=res.primal_value, gap=res.gap,
+                     primal_infeas=res.primal_infeas, err=res.err, iters=res.iters, outer=1, evals=res.evals,
+                     hvps=res.hvps, status=status, wall_s=time.perf_counter() - t0, history=[])
+
+
 def solve_pools(hp: HostPools, utility, nu0=None, tol: float = 1e-8, max_iter: int = 100, device="cuda",
                 verbose: bool = False, store: Optional[PoolStore] = None, want_trades: bool = True,
                 native=True, method: str = "auto", **solver_kw) -> Result:
@@ -241,7 +292,9 @@ def solve_pools(hp: HostPools, utility, nu0=None, tol: float = 1e-8, max_iter: i
     method: 'pools' = pool-parallel kernels under the outer loop (any size); 'thread' = the whole solve in one GPU
     thread (<= 64 tokens, arity <= 8); 'auto' picks 'thread' up to SMALL_POOLS pools.
     native (constant-product problems): True / 'persist' = the persistent solver kernel, 'hostloop' = the C++ host loop
-    over per-pass launches, False = the python loop (solver.py)."""
+    over per-pass launches, False = the python loop (solver.py).  native='hostloop' on any other single-GPU store (every
+    pool kind, mixed) runs the C++ market loop (cfmm_market_solve), which takes the solver_kw linear_solver, cg_max, eps,
+    eps_min, eps_shrink and max_outer; other keywords, or verbose, keep solver.py."""
     comm = Comm()
     if method not in ("auto", "pools", "thread"):
         raise ValueError("method must be 'auto', 'pools' or 'thread'")
@@ -266,6 +319,9 @@ def solve_pools(hp: HostPools, utility, nu0=None, tol: float = 1e-8, max_iter: i
                              impl="persist" if native is True else native)
         if want_trades:          # one more pass of the eval kernel to emit Delta / Lambda at the solution
             store.evaluate(info.nu, 0.0, trades=True, hess=False)
+    elif _market_applicable(store, native, verbose, solver_kw):
+        # any other single-GPU store: the C++ market loop; its final read-back already left the trades in the buckets
+        info = _solve_market(store, spec, nu0, tol, max_iter, **solver_kw)
     else:
         info = solve_dual(store, spec, nu0=nu0, tol=tol, max_inner=max_iter, comm=comm, verbose=verbose,
                           final_trades=want_trades, **solver_kw)

@@ -1638,6 +1638,19 @@ class PoolStore:
             if b.theta_bar is not None:
                 b.theta_bar.zero_()
 
+    def market_structs(self):
+        """The arguments of cfmm_market_solve that describe this store's pools: (plain cfmm_bucket array, their
+        cfmm_eval_out array (trades, hcoef, hmask), n_plain, the blocked bucket's cfmm_blocked_pairs or None, its
+        cfmm_eval_out (trades) or None).  The arrays point at this store's buffers; gather_trades() reads the trades of
+        the solve's final read-back."""
+        plain = [b for b in self.buckets if not getattr(b, "blocked", False)]
+        blk = [b for b in self.buckets if getattr(b, "blocked", False)]
+        buckets = (_lib.Bucket * max(len(plain), 1))(*[b.c_bucket for b in plain])
+        outs = (_lib.EvalOut * max(len(plain), 1))(*[b.out_struct(True, True) for b in plain])
+        if not blk:
+            return buckets, outs, len(plain), None, None
+        return buckets, outs, len(plain), blk[0].c_blocked, blk[0].out_struct(True, False)
+
     # -- a changed market: new reserves / fees in place ------------------------------------------------
     def _pool_map(self):
         """(bucket index or -1, position in that bucket) of every global pool id, built once per store"""

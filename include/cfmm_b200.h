@@ -305,6 +305,46 @@ int cfmm_blocked_solve_peer(const cfmm_blocked_pairs* b, int32_t n_tokens, const
                             const cfmm_solve_params* prm, cfmm_solve_result* res, cfmm_peer_ctx* peer, void* stream);
 
 /*
+ * Native outer loop (csrc/cfmm_solver.cu) for a market of ANY pool kinds on one GPU: the plain buckets
+ * buckets[0..n_buckets) of every CFMM_KIND_* cfmm_arb_eval takes, plus at most one blocked constant-product bucket
+ * (blocked, may be NULL).  The method of solver.py step for step: projected Newton on the dual, the Newton systems by
+ * Jacobi-PCG on Hessian-vector products or by a dense fp64 Cholesky (Levenberg-Marquardt ladder, active-set
+ * look-ahead up to n_tokens = 64), the method of multipliers on constant-sum fills (ramp eps0 -> eps_min by
+ * eps_shrink per outer pass, at most max_outer passes), and the final read-back: psi and the trades at the last eps,
+ * the dual value exact.  One difference: where no rung of the ladder factors, solver.py takes a least-squares step and
+ * this loop the steepest-descent one.  cfmm_blocked_solve is this loop's one-blocked-bucket case.
+ * outs[k]: bucket k's per-pool outputs, used as cfmm_arb_eval's `out`.  Every non-empty bucket needs hcoef, and hmask
+ * for GEOMEAN, STABLESWAP_N and CRYPTOSWAP_3 (CFMM_E_NULL otherwise); delta / lambda receive the trades of the final
+ * read-back (may be NULL, except lambda of a SUM bucket, whose theta_bar the loop resets and advances: CFMM_E_NULL).
+ * blocked_out: the blocked bucket's delta / lambda (blocked order), or NULL; its hcoef lives in `work`.
+ * Utility, c / a / eq / pinned / nu / psi_out and res as for cfmm_blocked_solve; `work`:
+ * cfmm_market_solve_work_bytes() bytes (same buckets, blocked, n_tokens and linear_solver).  Allocates no device memory;
+ * SYNCHRONOUS on `stream`.  CFMM_E_SIZE: n_tokens <= 0, n_buckets < 0, no pools at all, linear_solver outside 0..2,
+ * or a dense solve (forced, or chosen by auto) with n_tokens > 4096.  Nothing is launched when a check fails.
+ */
+typedef struct cfmm_market_params {   /* cfmm_solve_params is not changed (ABI) */
+    double tol, nu_floor;
+    double eps0, eps_min, eps_shrink;  /* constant-sum ramp continuation (solver.py: 0.1, 1e-4, 0.5)                   */
+    int32_t max_iter;                  /* Newton iterations per outer pass                                            */
+    int32_t cg_max;                    /* PCG iterations per Newton step                                              */
+    int32_t max_outer;                 /* method-of-multipliers passes (60)                                           */
+    int32_t linear_solver;             /* 0 auto (dense if n <= 256, or constant-sum pools and n <= 4096), 1 dense, 2 cg */
+} cfmm_market_params;
+
+int64_t cfmm_market_solve_work_bytes(const cfmm_bucket* buckets, int32_t n_buckets, const cfmm_blocked_pairs* blocked,
+                                     int32_t n_tokens, int32_t linear_solver);
+int cfmm_market_solve(const cfmm_bucket* buckets, const cfmm_eval_out* outs, int32_t n_buckets,
+                      const cfmm_blocked_pairs* blocked, const cfmm_eval_out* blocked_out, int32_t n_tokens,
+                      const double* c, const double* a, const uint8_t* eq, const uint8_t* pinned, double* nu,
+                      double* psi_out, void* work, const cfmm_market_params* prm, cfmm_solve_result* res, void* stream);
+
+/* The market loop's dense factorisation on its own: a (n x n, 1 <= n <= 4096, column-major; the lower triangle is
+ * read) becomes L (A = L L') in place, with the strictly lower part also mirrored into the upper triangle.  *info
+ * (device f64) = 0, or the 1-based index of the first pivot that is not positive and finite (then `a` is garbage).
+ * Asynchronous on `stream`. */
+int cfmm_dense_cholesky(int32_t n, double* a, double* info, void* stream);
+
+/*
  * The same solve (one GPU or sharded, same arguments and results) as ONE persistent cooperative kernel
  * (csrc/cfmm_persist.cu): every CTA keeps its chunk of pool tiles for the whole solve and runs all evaluation /
  * Hessian-product / diagonal passes on it; every CTA also owns slices of the n_tokens-long vectors and updates them
