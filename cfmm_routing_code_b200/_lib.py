@@ -11,6 +11,7 @@ from . import build as _build
 
 KIND_PRODUCT, KIND_SUM, KIND_GEOMEAN, KIND_BOUNDED, KIND_STABLESWAP, KIND_STABLESWAP_N, KIND_CONCENTRATED = 0, 1, 2, 3, 4, 5, 6
 KIND_CRYPTOSWAP, KIND_CRYPTOSWAP_3 = 8, 9
+KIND_BINS = 10
 
 _ERRORS = {
     -1: "CFMM_E_NULL (required pointer is NULL)",
@@ -181,10 +182,14 @@ def load(build_if_missing: bool = True):
     lib.cfmm_batch_solve_cryptoswap.restype = C.c_int
     lib.cfmm_batch_solve_tricrypto.argtypes = lib.cfmm_batch_solve_concentrated.argtypes
     lib.cfmm_batch_solve_tricrypto.restype = C.c_int
+    lib.cfmm_batch_solve_bins.argtypes = lib.cfmm_batch_solve_concentrated.argtypes
+    lib.cfmm_batch_solve_bins.restype = C.c_int
     lib.cfmm_allreduce_ll.argtypes = [vp, vp, i32, i32, i32, i64, i64, vp, C.c_uint64, vp]
     lib.cfmm_allreduce_ll.restype = C.c_int
     lib.cfmm_sum_update_multipliers.argtypes = [C.POINTER(Bucket), vp, vp, vp, vp]
     lib.cfmm_sum_update_multipliers.restype = C.c_int
+    lib.cfmm_bins_update_multipliers.argtypes = [C.POINTER(Bucket), vp, vp, vp, vp, vp]
+    lib.cfmm_bins_update_multipliers.restype = C.c_int
     lib.cfmm_zero.argtypes = [vp, i64, vp]
     lib.cfmm_zero.restype = C.c_int
     lib.cfmm_set_scatter_mode.argtypes = [i32]

@@ -14,7 +14,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .pools import HostPools, KIND_CONCENTRATED_HOST, KIND_CRYPTOSWAP_HOST, KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
+from .pools import HostPools, KIND_BINS_HOST, KIND_CONCENTRATED_HOST, KIND_CRYPTOSWAP_HOST, KIND_GEOMEAN_HOST, \
+    KIND_STABLESWAP_HOST
 from .solver import default_nu0
 
 NTOK_MAX = 64      # cfmm_small::NTOK_MAX
@@ -68,6 +69,19 @@ class CsrStore:
             self.logrw[first] = torch.as_tensor(lp[cl].astype(np.float64), device=dev)
             self.logrw[first + 1] = torch.as_tensor((lp[cl + 1] - lp[cl] - 1).astype(np.float64), device=dev)
             self.records = torch.as_tensor(np.ascontiguousarray(hp.lad_rec, np.float64).reshape(-1), device=dev)
+        bn = np.nonzero(np.asarray(hp.kind) == KIND_BINS_HOST)[0]
+        self.has_bins = bool(len(bn))                # -> cfmm_batch_solve_bins (a seventh instance)
+        if len(bn):                                  # bins pools: (z, p_ref) in the w slots, (first record, nb) in logrw;
+            first = torch.as_tensor(np.asarray(hp.pool_ptr)[bn], device=dev)   # their records after the ladders'
+            bp = np.asarray(hp.bin_ptr, np.int64)
+            n_lad = len(np.asarray(hp.lad_rec).reshape(-1, 4))
+            zp = np.asarray(hp.bin_zp, np.float64)[bn]
+            self.w[first] = torch.as_tensor(zp[:, 0], device=dev)
+            self.w[first + 1] = torch.as_tensor(zp[:, 1], device=dev)
+            self.logrw[first] = torch.as_tensor((bp[bn] + n_lad).astype(np.float64), device=dev)
+            self.logrw[first + 1] = torch.as_tensor((bp[bn + 1] - bp[bn]).astype(np.float64), device=dev)
+            self.records = torch.as_tensor(np.concatenate([np.asarray(hp.lad_rec, np.float64).reshape(-1),
+                                                           np.asarray(hp.bin_rec, np.float64).reshape(-1)]), device=dev)
         cs = np.nonzero(np.asarray(hp.kind) == KIND_CRYPTOSWAP_HOST)[0]
         ptr = np.asarray(hp.pool_ptr, np.int64)
         c3 = cs[ptr[cs + 1] - ptr[cs] == 3]
@@ -139,6 +153,10 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if store.has_bins:
+        _lib.check(store.lib.cfmm_batch_solve_bins(C.byref(store.c_pools), store.records.data_ptr(), C.byref(batch),
+                                                   C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve_bins")
+        return psi, stats, delta, lam
     if store.has_crypto3:
         _lib.check(store.lib.cfmm_batch_solve_tricrypto(C.byref(store.c_pools),
                                                         store.records.data_ptr() if store.records is not None else None,
@@ -218,6 +236,7 @@ def pack_problems(problems: Sequence):
     B = len(problems)
     ptr = [np.zeros(1, np.int64)]
     lptr = [np.zeros(1, np.int64)]               # concentrated records: their per-pool offsets shift like pool_ptr
+    bptr = [np.zeros(1, np.int64)]               # bins records likewise
     ranges = np.empty((B, 2), np.int64)
     c = np.zeros((B, n)); a = np.zeros((B, n)); fl = np.full((B, n), 2, np.uint8); nu = np.ones((B, n))
     m0, off0, nnz_max = 0, 0, 0
@@ -225,6 +244,7 @@ def pack_problems(problems: Sequence):
         hp.validate()
         ptr.append(np.asarray(hp.pool_ptr[1:], np.int64) + off0)
         lptr.append(np.asarray(hp.lad_ptr[1:], np.int64) + lptr[-1][-1])
+        bptr.append(np.asarray(hp.bin_ptr[1:], np.int64) + bptr[-1][-1])
         ranges[p] = (m0, m0 + hp.m)
         m0 += hp.m
         off0 += int(hp.pool_ptr[-1])
@@ -241,7 +261,9 @@ def pack_problems(problems: Sequence):
                        cat("amp", np.float64), cat("inv", np.float64), np.concatenate(lptr),
                        np.concatenate([np.asarray(hp.lad_rec, np.float64).reshape(-1, 4) for hp, _ in problems]),
                        np.concatenate([np.asarray(hp.lad_sc, np.float64).reshape(-1, 2) for hp, _ in problems]),
-                       cat("cgam", np.float64))
+                       cat("cgam", np.float64), np.concatenate(bptr),
+                       np.concatenate([np.asarray(hp.bin_rec, np.float64).reshape(-1, 4) for hp, _ in problems]),
+                       np.concatenate([np.asarray(hp.bin_zp, np.float64).reshape(-1, 2) for hp, _ in problems]))
     return merged, ranges, c, a, fl, nu, nnz_max
 
 

@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, os.environ.get("CFMM_LIB", "libcfmm_b200.so"))      # (CFMM_LIB: load / build an experiment variant)
 SOURCES = ["cfmm_kernels.cu", "cfmm_blocked.cu", "cfmm_layout.cu", "cfmm_persist.cu", "cfmm_solver.cu", "cfmm_allreduce.cu",
            "cfmm_small.cu", "cfmm_small_ladder.cu", "cfmm_splice.cu", "cfmm_small_crypto.cu",
-           "cfmm_small_tricrypto.cu"]
+           "cfmm_small_tricrypto.cu", "cfmm_small_bins.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",

@@ -9,7 +9,7 @@
 #include <math.h>
 
 #include "cfmm_dev.cuh"
-#include "cfmm_small.cuh"     // bounded_pair(), ladder_pair(), ...: the per-pool math, shared with the per-thread solver
+#include "cfmm_small.cuh"     // bounded_pair(), ladder_pair(), bins_pair(), ...: the per-pool math, shared with the per-thread solver
 
 namespace cfmm {
 std::atomic<long long> g_launches{0};
@@ -260,6 +260,40 @@ k_eval_ladder(long long m, long long ld, int n_tokens, const int* __restrict__ i
         double D[2], L[2], h;
         cfmm_small::ladder_pair(rec + 4 * (long long)P[2 * ld + i], (long long)P[3 * ld + i], (long long)P[ld + i], P[i],
                                 gamma[i], n0, n1, D, L, h);
+        const double y0 = L[0] - D[0], y1 = L[1] - D[1];
+        if (TRADES) {
+            delta[i] = D[0]; delta[ld + i] = D[1];
+            lambda[i] = L[0]; lambda[ld + i] = L[1];
+        }
+        if (HESS) hcoef[i] = h;
+        if (y0 != 0.0) sc.add(i0, y0);
+        if (y1 != 0.0) sc.add(i1, y1);
+        acc += n0 * y0 + n1 * y1;
+    }
+    sc.flush(smem, n_tokens);
+    block_accumulate(acc, arb);
+}
+
+// price bins (Liquidity Book bins, order books, limit orders): cfmm_small::bins_pair, one thread per pool.  rec = the
+// AoS records (the bucket's weights), P [4][ld] = (first record, nb, z, p_ref) (the bucket's logrw), tbar = theta_bar
+// row 0 (read only when eps > 0).  The reserves are not read.  A trade that stays in the segment next to t = 0 reads
+// O(1) records; one that crosses k breakpoints O(log k) more.
+template <typename Scatter, bool TRADES, bool HESS>
+__global__ void __launch_bounds__(kThreads)
+k_eval_bins(long long m, long long ld, int n_tokens, const int* __restrict__ idx, const double* __restrict__ gamma,
+            const double* __restrict__ rec, const double* __restrict__ P, const double* __restrict__ tbar, double eps,
+            const double* __restrict__ nu, double* psi, double* arb, double* delta, double* lambda, double* hcoef) {
+    extern __shared__ double smem[];
+    Scatter sc{psi};
+    sc.init(smem, n_tokens);
+    double acc = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        const int i0 = idx[i], i1 = idx[ld + i];
+        const double n0 = __ldg(nu + i0), n1 = __ldg(nu + i1);
+        double D[2], L[2], h;
+        cfmm_small::bins_pair(rec + 4 * (long long)P[i], (long long)P[ld + i], (long long)P[2 * ld + i], P[3 * ld + i],
+                              eps > 0.0 ? tbar[i] : 0.0, gamma[i], n0, n1, eps, D, L, h);
         const double y0 = L[0] - D[0], y1 = L[1] - D[1];
         if (TRADES) {
             delta[i] = D[0]; delta[ld + i] = D[1];
@@ -831,6 +865,26 @@ k_sum_update(long long m, long long ld, const double* __restrict__ R, const doub
     }
 }
 
+// price bins: tbar <- t = lambda_0 - delta_0 (row 0 of theta_bar; row 1 is not used), move = max |change| / S with S
+// the width of the pool's net-flow domain at its fee
+__global__ void __launch_bounds__(kThreads)
+k_bins_update(long long m, long long ld, const double* __restrict__ rec, const double* __restrict__ P,
+              const double* __restrict__ gamma, const double* __restrict__ delta, const double* __restrict__ lambda,
+              double* thbar, double* move) {
+    double mx = 0.0;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += stride) {
+        const double* rp = rec + 4 * (long long)P[i];
+        const double S = rp[4 * ((long long)P[ld + i] - 1)] - rp[0] / gamma[i];
+        const double t = lambda[i] - delta[i];
+        mx = fmax(mx, fabs(t - thbar[i]) / S);
+        thbar[i] = t;
+    }
+    mx = warp_max(mx);
+    if ((threadIdx.x & 31) == 0 && mx > 0.0)
+        atomicMax(reinterpret_cast<unsigned long long*>(move), (unsigned long long)__double_as_longlong(mx));
+}
+
 // ---------------------------------------------------------------------------------------------
 // launch helpers
 // ---------------------------------------------------------------------------------------------
@@ -1028,11 +1082,35 @@ int launch_ladder(const cfmm_bucket* b, int n_tokens, const double* nu, double* 
     return check_launch();
 }
 
+// price-bin buckets: the LDG path only, like the concentrated kind
+template <bool TRADES, bool HESS>
+int launch_bins(const cfmm_bucket* b, int n_tokens, const double* nu, double eps, double* psi, double* arb,
+                const cfmm_eval_out* out, cudaStream_t st) {
+    const long long m = b->n_pools;
+    double* delta = out ? out->delta : nullptr;
+    double* lambda = out ? out->lambda : nullptr;
+    double* hcoef = out ? out->hcoef : nullptr;
+    if (use_shared(n_tokens, m)) {
+        const size_t sm = (size_t)n_tokens * sizeof(double);
+        auto kern = k_eval_bins<SharedScatter, TRADES, HESS>;
+        allow_smem(kern, sm);
+        kern<<<grid_for(m, 2), kThreads, sm, st>>>(m, b->stride, n_tokens, b->tok_idx, b->gamma, b->weights, b->logrw,
+                                                    b->theta_bar, eps, nu, psi, arb, delta, lambda, hcoef);
+    } else {
+        k_eval_bins<GlobalScatter, TRADES, HESS><<<grid_for(m, 8), kThreads, 0, st>>>(
+            m, b->stride, n_tokens, b->tok_idx, b->gamma, b->weights, b->logrw, b->theta_bar, eps, nu, psi, arb, delta,
+            lambda, hcoef);
+    }
+    return check_launch();
+}
+
 template <int KIND, bool TRADES, bool HESS>
 int launch_kind(const cfmm_bucket* b, int n_tokens, const double* nu, double eps, double* psi, double* arb,
                 const cfmm_eval_out* out, cudaStream_t st) {
     if constexpr (KIND == CFMM_KIND_CONCENTRATED)
         return launch_ladder<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
+    else if constexpr (KIND == CFMM_KIND_BINS)
+        return launch_bins<TRADES, HESS>(b, n_tokens, nu, eps, psi, arb, out, st);
     else if constexpr (KIND == CFMM_KIND_STABLESWAP)
         return launch_stable<TRADES, HESS>(b, n_tokens, nu, psi, arb, out, st);
     else if constexpr (KIND == CFMM_KIND_CRYPTOSWAP)
@@ -1123,6 +1201,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 3) return CFMM_E_KIND;
             if (b->n_pools > 0 && (!b->weights || !b->logrw)) return CFMM_E_NULL;   // price scales; (A, G, D)
             break;
+        case CFMM_KIND_BINS:
+            if (b->arity != 2) return CFMM_E_KIND;
+            if (b->n_pools > 0 && (!b->weights || !b->logrw || !b->theta_bar)) return CFMM_E_NULL;   // records; tbar
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -1156,6 +1238,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_CONCENTRATED>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_CRYPTOSWAP:
             return dispatch_pair<CFMM_KIND_CRYPTOSWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_BINS:
+            return dispatch_pair<CFMM_KIND_BINS>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_CRYPTOSWAP_3:
             return dispatch_crypto3(b, n_tokens, nu, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP_N:
@@ -1292,6 +1376,18 @@ int cfmm_sum_update_multipliers(const cfmm_bucket* b, const double* lambda, doub
     if (!lambda || !theta_bar_out || !move || !b->reserves) return CFMM_E_NULL;
     k_sum_update<<<grid_for(2 * b->n_pools, 8), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
         b->n_pools, b->stride, b->reserves, lambda, theta_bar_out, move);
+    return check_launch();
+}
+
+int cfmm_bins_update_multipliers(const cfmm_bucket* b, const double* delta, const double* lambda, double* theta_bar_out,
+                                 double* move, void* stream) {
+    if (!b) return CFMM_E_NULL;
+    if (b->kind != CFMM_KIND_BINS || b->arity != 2) return CFMM_E_KIND;
+    if (b->n_pools < 0 || b->stride < b->n_pools) return CFMM_E_SIZE;
+    if (b->n_pools == 0) return CFMM_OK;
+    if (!delta || !lambda || !theta_bar_out || !move || !b->weights || !b->logrw || !b->gamma) return CFMM_E_NULL;
+    k_bins_update<<<grid_for(b->n_pools, 8), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        b->n_pools, b->stride, b->weights, b->logrw, b->gamma, delta, lambda, theta_bar_out, move);
     return check_launch();
 }
 

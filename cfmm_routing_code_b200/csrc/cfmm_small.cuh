@@ -191,6 +191,82 @@ CFMM_HD inline void ladder_pair(const double* rec, int64_t T, int64_t c, double 
     }
 }
 
+// Price-bin pool (Liquidity Book bins, an order book, limit orders): bins k at prices p_k (token 1 per token 0) holding
+// x_k of token 0 and y_k of token 1, uncrossed (every bin with y > 0 prices at or below every bin with x > 0); its
+// trading set is the Minkowski sum of the bins' constant-sum sets.  In net-flow form the pool pays out t of token 0 for
+// the least C(t) of token 1, C convex piecewise linear: slope p_k / gamma over x_k for t > 0 (asks, ascending), slope
+// gamma p_k over y_k / (gamma p_k) for t < 0 (bids, descending).  One fee-free record per breakpoint j = 0 .. nb - 1,
+// ascending in t, rec[4j .. 4j+3] = {T_j, C_j, q_j, bin}: record z is (0, 0); above it T is the cumulative x and C the
+// cumulative p x of the asks, below it T is minus the cumulative y / p and C minus the cumulative y of the bids, both
+// accumulated outward from t = 0; q_j = the price of the segment (j, j+1) and bin its bin (0 and -1 on the last record).
+// The fee is applied here: breakpoint j is at (T_j / gamma, C_j) below z and (T_j, C_j / gamma) above it.
+// Exact (eps <= 0): t* maximises r t - C(t), r = nu0 / nu1, a breakpoint; a segment fills only when strictly profitable
+// (sum_order's rule).  Smoothed (eps > 0): t maximises r t - C(t) - (t - tbar)^2 / (2 a), a = sigma / p_ref, sigma =
+// S / eps, S = the width of C's domain; the trader pays the smoothing term, so the trade stays pool-feasible.
+// Flows (+t, -(C(t) + smoothing)); hc = a r nu0 inside a segment, 0 at a breakpoint or an end.  The end breakpoint is
+// the largest j whose left end of the subgradient of t + a C'(t) is <= tbar + a r (exact: whose left segment fills),
+// found by an exponential search outward from z and a bisection, O(log |j - z|) record reads, fixed loop bounds.
+// Returns t.  Shared by the per-thread solver and k_eval_bins (cfmm_kernels.cu).
+constexpr int64_t BINS_K_MAX = int64_t(1) << 20;     // most bins of one pool (pools.BINS_K_MAX): nb <= K + 2
+
+CFMM_HD inline double bins_slope(const double* rec, int64_t j, int64_t z, double gam) {   // segment (j, j+1)
+    return j < z ? gam * rec[4 * j + 2] : rec[4 * j + 2] / gam;
+}
+
+CFMM_HD inline double bins_pair(const double* rec, int64_t nb, int64_t z, double pref, double tbar, double gam,
+                                double n0, double n1, double eps, double* D, double* L, double& hc) {
+    D[0] = D[1] = L[0] = L[1] = 0.0;
+    hc = 0.0;
+    const double r = n0 / n1;
+    const double tlo = rec[0] / gam, thi = rec[4 * (nb - 1)];
+    const double a = eps > 0.0 ? (thi - tlo) / (eps * pref) : 0.0;
+    auto tat = [&](int64_t j) { return j < z ? rec[4 * j] / gam : rec[4 * j]; };
+    auto cat = [&](int64_t j) { return j > z ? rec[4 * j + 1] / gam : rec[4 * j + 1]; };
+    // pred(j): breakpoint j is at or below the solution; true at j = 0, monotone (true ... false)
+    auto pred = [&](int64_t j) {
+        if (j <= 0) return true;
+        if (eps > 0.0) return tat(j) - tbar <= a * (r - bins_slope(rec, j - 1, z, gam));
+        return j <= z ? !(r < gam * rec[4 * (j - 1) + 2]) : gam * r > rec[4 * (j - 1) + 2];
+    };
+    int64_t lo, hi;                                                    // pred(lo), !pred(hi) (hi = nb: past the top)
+    if (pred(z)) {
+        lo = z; hi = nb;
+        for (int it = 0, step = 1; it < LADDER_SEARCH; ++it, step *= 2) {
+            const int64_t c = lo + step < nb ? lo + step : nb;
+            if (c >= nb || !pred(c)) { hi = c; break; }
+            lo = c;
+        }
+    } else {
+        hi = z; lo = 0;
+        for (int it = 0, step = 1; it < LADDER_SEARCH; ++it, step *= 2) {
+            const int64_t c = hi - step > 0 ? hi - step : 0;
+            if (pred(c)) { lo = c; break; }
+            hi = c;
+        }
+    }
+    for (int it = 0; it < LADDER_SEARCH; ++it) {
+        if (hi - lo <= 1) break;
+        const int64_t mid = lo + (hi - lo) / 2;
+        if (pred(mid)) lo = mid; else hi = mid;
+    }
+    const int64_t j = lo;
+    double t = tat(j), C = cat(j);
+    if (eps > 0.0 && j < nb - 1) {
+        const double s = bins_slope(rec, j, z, gam);
+        const double w = tbar + a * (r - s);
+        if (w > t) {                                                   // inside segment (j, j+1)
+            t = fmin(w, tat(j + 1));
+            C = j < z ? cat(j + 1) + s * (t - tat(j + 1)) : C + s * (t - tat(j));
+            if (t < tat(j + 1)) hc = a * r * n0;
+        }
+    }
+    const double sm = eps > 0.0 ? (t - tbar) * (t - tbar) / (2.0 * a) : 0.0;
+    const double y1 = -(C + sm);
+    L[0] = fmax(t, 0.0); D[0] = fmax(-t, 0.0);
+    L[1] = fmax(y1, 0.0); D[1] = fmax(-y1, 0.0);
+    return t;
+}
+
 // Two-coin StableSwap (Curve) pool: scaled balances y_j = r_j x_j on the invariant
 //     4A (y0 + y1) + D = 4A D + D^3 / (4 y0 y1),        D = the invariant of the current reserves (precomputed),
 // worked in units of D (u_j = y_j / D, so 4A (u0 + u1) + 1 = 4A + 1 / (4 u0 u1)) so nothing overflows.  Along the curve
@@ -900,8 +976,11 @@ CFMM_UNROLL
 // CRYPTO3 (with all four): also three-coin cryptoswap pools (kind 9) through cryptoswap3, c_j = p_j / D in the pool's
 // three w slots and (A, G) in its first two logrw slots, the Hessian block added from the three edge weights;
 // cfmm_batch_solve_tricrypto runs this sixth instance.  The other instances give problems with such pools status 3.
+// BINS (with all five): also price-bin pools (kind 10) through bins_pair, (z, p_ref) in the pool's two w slots, (first
+// record, nb) in its two logrw slots, the records in `rec` (shared with the concentrated pools') and the multiplier tbar in
+// its first theta_bar slot; cfmm_batch_solve_bins runs this seventh instance.  The others give such problems status 3.
 template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
-          bool CRYPTO3 = false>
+          bool CRYPTO3 = false, bool BINS = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane,
                                const double* rec = nullptr) {
@@ -935,6 +1014,17 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
             double hc = 0.0;
             cryptoswap_pair(P.R[off], P.R[off + 1], P.w[off], P.w[off + 1], P.logrw[off], P.logrw[off + 1], gam,
                             nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
+            if (Hs && hc != 0.0) {
+                const int t0 = P.tok[off], t1 = P.tok[off + 1];
+                (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
+                (*Hs)[t0 * n + t1] -= hc; (*Hs)[t1 * n + t0] -= hc;
+            }
+        } else if (BINS && P.kind[i] == 10) {                 // (z, p_ref) in w, (first record, nb) in logrw, tbar in theta_bar
+            double hc = 0.0;
+            const double t = bins_pair(rec + 4 * (int64_t)P.logrw[off], (int64_t)P.logrw[off + 1], (int64_t)P.w[off],
+                                       P.w[off + 1], eps > 0.0 ? Q.theta_bar[off - Q.off0] : 0.0, gam, nu[P.tok[off]],
+                                       nu[P.tok[off + 1]], eps, D, L, hc);
+            if (store_fill) { Q.theta_new[off - Q.off0] = t; Q.theta_new[off - Q.off0 + 1] = 0.0; }
             if (Hs && hc != 0.0) {
                 const int t0 = P.tok[off], t1 = P.tok[off + 1];
                 (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
@@ -1167,9 +1257,9 @@ CFMM_HD inline int newton_direction(int n, uint64_t free_mask, const Vec& Hs, co
 CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL * n * n + (int64_t)n * (n + 1) + 2 * nnz; }
 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
-// rec: the concentrated pools' records (LADDER instance only).
+// rec: the concentrated and price-bin pools' records (LADDER and BINS instances only).
 template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
-          bool CRYPTO3 = false>
+          bool CRYPTO3 = false, bool BINS = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0, const double* rec = nullptr) {
     const int n = Q.n;
@@ -1188,11 +1278,12 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     for (int64_t i = Q.p0; i < Q.p1 && !bad; ++i) {                         // refuse what the closed forms do not cover
         const int64_t o = P.pool_ptr[i];
         const int k = (int)(P.pool_ptr[i + 1] - o);
-        has_sum = has_sum || P.kind[i] == 1;
+        has_sum = has_sum || P.kind[i] == 1 || (BINS && P.kind[i] == 10);
         bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6) && !(CRYPTO && P.kind[i] == 8) &&
-               !(CRYPTO3 && P.kind[i] == 9)) || k < 2 ||
+               !(CRYPTO3 && P.kind[i] == 9) && !(BINS && P.kind[i] == 10)) || k < 2 ||
               k > KMAX || ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
-                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8)) && k != 2) || (CRYPTO3 && P.kind[i] == 9 && k != 3);
+                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8) || (BINS && P.kind[i] == 10)) && k != 2) ||
+              (CRYPTO3 && P.kind[i] == 9 && k != 3);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
     if (bad) {
@@ -1219,7 +1310,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -1265,7 +1356,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -1290,8 +1381,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -1304,6 +1395,14 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         failed_before = inner_status != 0;
         move = 0.0;
         for (int64_t i = Q.p0; i < Q.p1; ++i) {
+            if (BINS && P.kind[i] == 10) {                               // tbar <- t; move relative to the domain width
+                const int64_t o = P.pool_ptr[i] - Q.off0;
+                const double* rp = rec + 4 * (int64_t)P.logrw[P.pool_ptr[i]];
+                const double S = rp[4 * ((int64_t)P.logrw[P.pool_ptr[i] + 1] - 1)] - rp[0] / P.gamma[i];
+                move = fmax(move, fabs(Q.theta_new[o] - Q.theta_bar[o]) / S);
+                Q.theta_bar[o] = Q.theta_new[o];
+                continue;
+            }
             if (P.kind[i] != 1) continue;
             const int64_t o = P.pool_ptr[i] - Q.off0;
             for (int b = 0; b < 2; ++b) {
@@ -1316,8 +1415,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

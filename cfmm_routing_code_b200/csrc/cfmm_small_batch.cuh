@@ -1,7 +1,8 @@
 // cfmm_small_batch.cuh -- the per-thread batch solver's kernel body, shared by the translation units that instantiate it
 // (cfmm_small.cu: the plain and StableSwap instances; cfmm_small_ladder.cu: the concentrated one; cfmm_small_crypto.cu:
-// the cryptoswap one; cfmm_small_tricrypto.cu: the three-coin cryptoswap one).  Each includer gets its
-// own copy in an anonymous namespace; the lane setting and the argument checks live in cfmm_small.cu.
+// the cryptoswap one; cfmm_small_tricrypto.cu: the three-coin cryptoswap one; cfmm_small_bins.cu: the price-bin one).
+// Each includer gets its own copy in an anonymous namespace; the lane setting and the argument checks live in
+// cfmm_small.cu.
 #pragma once
 #include "cfmm_dev.cuh"
 #include "cfmm_small.cuh"
@@ -22,8 +23,9 @@ constexpr int kSmallThreads = 32;     // one warp per CTA: a sweep of 50 problem
 // STABLE: also evaluate StableSwap pools (k_batch_solve_stable); without it such a pool makes its problem status 3.
 // STABLE_N: StableSwap pools of 2..8 coins (k_batch_solve_stable_n).  LADDER: concentrated pools too, their records in
 // `rec` (k_batch_solve_ladder).  CRYPTO: two-coin cryptoswap pools too (k_batch_solve_crypto).  CRYPTO3: three-coin
-// cryptoswap pools too (k_batch_solve_tricrypto).
-template <int LANES, bool STABLE, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false, bool CRYPTO3 = false>
+// cryptoswap pools too (k_batch_solve_tricrypto).  BINS: price-bin pools too (k_batch_solve_bins).
+template <int LANES, bool STABLE, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false, bool CRYPTO3 = false,
+          bool BINS = false>
 __device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, const cfmm_batch& B, const cfmm_small::Params& prm,
                                                  int n, long long n_pools, double* work, long long stride,
                                                  const double* rec = nullptr) {
@@ -49,7 +51,7 @@ __device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, con
     Q.flags = B.flags + p * n;
     Q.delta = B.delta ? B.delta + p * B.trade_stride : nullptr;
     Q.lam = B.lambda ? B.lambda + p * B.trade_stride : nullptr;
-    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3>(
+    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(
         P, Q, prm, B.nu + p * n, B.psi + p * n, work + (LANES == 1 ? p : p * LANES + lane), stride, lane, rec);
     if (lane == 0) {
         st[0] = r.value; st[1] = r.dual; st[2] = r.gap; st[3] = r.infeas; st[4] = r.err;

@@ -555,7 +555,7 @@ int run_loop(const Market& mk, int n, const double* c, const double* a, const ui
     k_bounds<<<1, kVT, 0, st>>>(n, c, eq, pinned, cfg.nu_floor, lb, nu);
     if (mk.has_sum)                                     // solver.py: ev.reset_multipliers()
         for (int k = 0; k < mk.nb; ++k)
-            if (mk.b[k].kind == CFMM_KIND_SUM && mk.b[k].n_pools > 0)
+            if ((mk.b[k].kind == CFMM_KIND_SUM || mk.b[k].kind == CFMM_KIND_BINS) && mk.b[k].n_pools > 0)
                 cudaMemsetAsync(const_cast<double*>(mk.b[k].theta_bar), 0, 8 * 2 * (size_t)mk.b[k].stride, st);
     // evaluate at `x` into acc[ai]; returns the buffer used.  The calls and their order are PoolStore.evaluate's.
     auto eval = [&](const double* x, double eps, int what) -> double* {
@@ -753,6 +753,9 @@ int run_loop(const Market& mk, int n, const double* c, const double* a, const ui
             if (mk.b[k].kind == CFMM_KIND_SUM)
                 rc = cfmm_sum_update_multipliers(&mk.b[k], mk.outs[k].lambda, const_cast<double*>(mk.b[k].theta_bar),
                                                  V.sc + S_MOVE, st);
+            else if (mk.b[k].kind == CFMM_KIND_BINS)
+                rc = cfmm_bins_update_multipliers(&mk.b[k], mk.outs[k].delta, mk.outs[k].lambda,
+                                                  const_cast<double*>(mk.b[k].theta_bar), V.sc + S_MOVE, st);
         if (rc) return rc;
         if (!fetch()) return CFMM_E_CUDA;
         move = hsc[S_MOVE];
@@ -816,10 +819,11 @@ int check_market(const cfmm_bucket* buckets, const cfmm_eval_out* outs, int32_t 
         if (b.kind == CFMM_KIND_GEOMEAN) mk->has_geo = true;
         if (b.n_pools == 0) continue;
         pools += b.n_pools;
-        if (b.kind == CFMM_KIND_SUM) mk->has_sum = true;
+        if (b.kind == CFMM_KIND_SUM || b.kind == CFMM_KIND_BINS) mk->has_sum = true;
         if (!outs) continue;
         if (!outs[k].hcoef || (uses_hmask(b.kind) && !outs[k].hmask)) return CFMM_E_NULL;
         if (b.kind == CFMM_KIND_SUM && (!outs[k].lambda || !b.theta_bar)) return CFMM_E_NULL;
+        if (b.kind == CFMM_KIND_BINS && (!outs[k].delta || !outs[k].lambda || !b.theta_bar)) return CFMM_E_NULL;
     }
     if (pools == 0) return CFMM_E_SIZE;
     *dense = resolve_dense(linear_solver, n_tokens, mk->has_sum);

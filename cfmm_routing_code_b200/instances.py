@@ -537,3 +537,190 @@ def synth_tricrypto_market(m, n_tokens, seed, frac_tri=0.3, far=0.5, mispricing=
                    np.concatenate([base.lad_ptr, np.full(n_t, base.lad_ptr[-1], np.int64)]), base.lad_rec,
                    np.concatenate([base.lad_sc, np.zeros((n_t, 2))]), np.concatenate([np.asarray(base.cgam, float), G]))
     return hp, p
+
+
+LB_ID_OFFSET = 1 << 23      # Liquidity Book's bin id of price 1 (raw units)
+
+
+def lb_bins(active_id, bin_step, ids, reserves_x, reserves_y, decimals_x, decimals_y):
+    """A Liquidity Book (LFJ / Trader Joe v2.x) pair's bins as the (prices, x, y) of HostPools.from_lists' 'bins' kind:
+    bin id k trades at (1 + bin_step / 1e4)^(k - 2^23) raw Y per raw X, so at (1 + bin_step / 1e4)^(k - 2^23) *
+    10^(decimals_x - decimals_y) token Y per token X, computed in 40-digit decimal and rounded once; holdings are the raw
+    reserves over 10^decimals.  Token X is the pool's token 0.  Bins above active_id must hold no Y and bins below it no
+    X (ValueError otherwise); the rules of from_lists apply to the result.  The fee is the caller's (LB's variable and
+    composition fees are not modelled)."""
+    import decimal
+    ids = np.asarray(ids, np.int64).reshape(-1)
+    rx, ry = np.asarray(reserves_x, object).reshape(-1), np.asarray(reserves_y, object).reshape(-1)
+    if not (len(ids) == len(rx) == len(ry)) or len(ids) == 0:
+        raise ValueError("lb_bins: one reserve of each token per bin id")
+    if not 1 <= int(bin_step) <= 10000:
+        raise ValueError("lb_bins: bin_step must be 1 .. 10000 basis points")
+    o = np.argsort(ids, kind="stable")
+    ids, rx, ry = ids[o], rx[o], ry[o]
+    if np.any(np.diff(ids) <= 0):
+        raise ValueError("lb_bins: bin ids must be distinct")
+    if any(int(v) < 0 for v in rx) or any(int(v) < 0 for v in ry):
+        raise ValueError("lb_bins: reserves must be >= 0")
+    if any(int(rx[k]) > 0 for k in np.nonzero(ids < active_id)[0]) or \
+            any(int(ry[k]) > 0 for k in np.nonzero(ids > active_id)[0]):
+        raise ValueError("lb_bins: bins below the active one hold only Y, bins above it only X")
+    with decimal.localcontext() as ctx:
+        ctx.prec = 40
+        D = decimal.Decimal
+        base = D(1) + D(int(bin_step)) / D(10000)
+        scale = D(10) ** (int(decimals_x) - int(decimals_y))
+        prices = np.array([float(base ** (int(k) - LB_ID_OFFSET) * scale) for k in ids.tolist()])
+        x = np.array([float(D(int(v)) / D(10) ** int(decimals_x)) for v in rx])
+        y = np.array([float(D(int(v)) / D(10) ** int(decimals_y)) for v in ry])
+    return prices, x, y
+
+
+def order_book(bids, asks):
+    """An order book (or a batch of limit orders) as the (prices, x, y) of HostPools.from_lists' 'bins' kind: bids and
+    asks are (price, size) levels, price in token 1 per token 0, size in token 0.  An ask is a bin holding x = size at
+    its price; a bid one holding y = price * size; equal prices merge (a bid and an ask at the same price share a bin).
+    A crossed book (a bid above an ask) raises ValueError."""
+    lv = {}
+    for side, levels in ((1, bids), (0, asks)):
+        for pr, sz in levels:
+            pr, sz = float(pr), float(sz)
+            if not (np.isfinite(pr) and pr > 0 and np.isfinite(sz) and sz >= 0):
+                raise ValueError("order_book: prices must be finite and > 0, sizes finite and >= 0")
+            e = lv.setdefault(pr, [0.0, 0.0])
+            e[side] += pr * sz if side else sz
+    if not lv:
+        raise ValueError("order_book: no levels")
+    prices = np.array(sorted(lv))
+    x = np.array([lv[p][0] for p in prices]); y = np.array([lv[p][1] for p in prices])
+    if x.any() and y.any() and prices[y > 0].max() > prices[x > 0].min():
+        raise ValueError("order_book: the book is crossed (a bid above an ask)")
+    return prices, x, y
+
+
+def bins_split(hp):
+    """The same market with every bins pool written as its bins, one one-bin 'bins' pool each (the active bin keeps both
+    holdings) at the pool's fee, holdings read back from the records (x = the width of an ask segment, y = minus the
+    rise of C over a bid segment).  In exact arithmetic the two forms trade the same: a bins pool's trading set is the
+    Minkowski sum of its bins'.  The other pools keep their order and come first, the one-bin pools follow in pool and
+    price order.  Returns (HostPools, owner): owner[j] = the pool of hp that pool j of the result comes from."""
+    from .pools import HostPools, KIND_BINS_HOST
+    kind = np.asarray(hp.kind)
+    ptr = np.asarray(hp.pool_ptr, np.int64)
+    bn = kind == KIND_BINS_HOST
+    keep = np.nonzero(~bn)[0]
+    ar = np.diff(ptr)
+    slots = np.repeat(ptr[keep], ar[keep]) + (np.arange(int(ar[keep].sum())) - np.repeat(
+        np.concatenate([[0], np.cumsum(ar[keep])[:-1]]), ar[keep])) if len(keep) else np.zeros(0, np.int64)
+    bp = np.asarray(hp.bin_ptr, np.int64)
+    rec = np.asarray(hp.bin_rec, np.float64).reshape(-1, 4)
+    cnt = np.diff(bp)
+    owner_r = np.repeat(np.arange(hp.m), cnt)
+    last = np.zeros(len(rec), bool); last[bp[1:][cnt > 0] - 1] = True
+    seg = np.nonzero(~last)[0]                                       # every segment of every bins pool
+    o = owner_r[seg]
+    ask = (seg - bp[o]) >= np.asarray(hp.bin_zp, float)[o, 0]
+    x = np.where(ask, rec[seg + 1, 0] - rec[seg, 0], 0.0)
+    y = np.where(ask, 0.0, rec[seg + 1, 1] - rec[seg, 1])
+    new = np.ones(len(seg), bool)                                    # the active bin's two segments become one pool
+    new[1:] = (o[1:] != o[:-1]) | (rec[seg[1:], 3] != rec[seg[:-1], 3])
+    gid = np.cumsum(new) - 1
+    ng = int(gid[-1]) + 1 if len(seg) else 0
+    xg, yg = np.bincount(gid, x, ng), np.bincount(gid, y, ng)
+    first = seg[new]
+    og, pg, bg = o[new], rec[first, 2], rec[first, 3]
+    hy, hx = yg > 0, xg > 0
+    nrec = 2 + (hx & hy)
+    st = np.concatenate([[0], np.cumsum(nrec)[:-1]]).astype(np.int64)
+    zg = hy.astype(np.int64)
+    out_rec = np.zeros((int(nrec.sum()), 4))
+    out_rec[st[hy]] = np.stack([-yg[hy] / pg[hy], -yg[hy], pg[hy], bg[hy]], 1)
+    out_rec[st + zg, 2] = np.where(hx, pg, 0.0)
+    out_rec[st + zg, 3] = np.where(hx, bg, -1.0)
+    out_rec[st[hx] + zg[hx] + 1] = np.stack([xg[hx], pg[hx] * xg[hx], np.zeros(hx.sum()), np.full(hx.sum(), -1.0)], 1)
+    M = len(keep) + ng
+    new_ar = np.concatenate([ar[keep], np.full(ng, 2)])
+    lad_ptr = np.concatenate([np.asarray(hp.lad_ptr, np.int64)[keep], np.full(ng + 1, np.asarray(hp.lad_ptr)[-1])])
+    bin_ptr = np.zeros(M + 1, np.int64); bin_ptr[len(keep) + 1:] = np.cumsum(nrec)
+    bin_zp = np.zeros((M, 2)); bin_zp[len(keep):, 0], bin_zp[len(keep):, 1] = zg, pg
+    tok = np.asarray(hp.tok_idx)
+    out = HostPools(hp.n_tokens, np.concatenate([[0], np.cumsum(new_ar)]).astype(np.int64),
+                    np.concatenate([tok[slots], np.stack([tok[ptr[og]], tok[ptr[og] + 1]], 1).ravel()]).astype(np.int32),
+                    np.concatenate([np.asarray(hp.reserves)[slots], np.stack([xg, yg], 1).ravel()]),
+                    np.concatenate([np.asarray(hp.weights)[slots], np.zeros(2 * ng)]),
+                    np.concatenate([np.asarray(hp.gamma)[keep], np.asarray(hp.gamma)[og]]),
+                    np.concatenate([kind[keep], np.full(ng, KIND_BINS_HOST)]).astype(np.uint8),
+                    np.concatenate([np.asarray(hp.amp)[keep], np.zeros(ng)]),
+                    np.concatenate([np.asarray(hp.inv)[keep], np.zeros(ng)]),
+                    lad_ptr, hp.lad_rec, np.concatenate([np.asarray(hp.lad_sc).reshape(-1, 2)[keep], np.zeros((ng, 2))]),
+                    np.concatenate([np.asarray(hp.cgam)[keep], np.zeros(ng)]), bin_ptr, out_rec, bin_zp)
+    return out, np.concatenate([keep, og]).astype(np.int64)
+
+
+def synth_bins_market(m, n_tokens, seed, K=(1, 256), frac_lb=0.3, frac_book=0.1, frac_order=0.1, mispricing=0.02):
+    """A market of price-bin pools beside constant-product pools: m pools, a frac_lb share Liquidity-Book-like pools on
+    bin steps of 1 .. 100 bp with K bins (an int, or a (lo, hi) range drawn log-uniformly) around an active bin that
+    holds both tokens, their liquidity shaped like a bell around it (spot) or flat (a wide range); a frac_book share
+    order books (a spread of 2 .. 20 bp around the mid, K levels split between the sides, sizes log-normal); a
+    frac_order share single limit orders (one bin holding one token, at up to 1 % through the price, fee 1); the rest
+    constant product.  The mid of every bins pool is mispriced by `mispricing`.  Returns (HostPools, prices)."""
+    from .pools import HostPools, KIND_BINS_HOST, KIND_GEOMEAN_HOST, bin_records
+    rng = np.random.default_rng(seed)
+    n_lb, n_book, n_ord = (int(round(f * m)) for f in (frac_lb, frac_book, frac_order))
+    n_bins = n_lb + n_book + n_ord
+    base = synth_const_product(m - n_bins, n_tokens, seed, mispricing=mispricing)
+    p = base["prices"]
+    a = rng.integers(0, n_tokens, n_bins)
+    b = (a + rng.integers(1, n_tokens, n_bins)) % n_tokens
+    mid = p[a] / p[b] * np.exp(mispricing * rng.standard_normal(n_bins))
+    if np.ndim(K) == 0:
+        Ks = np.full(n_bins, int(K))
+    else:
+        Ks = np.exp(rng.uniform(np.log(K[0]), np.log(K[1] + 1), n_bins)).astype(np.int64).clip(K[0], K[1])
+    value = np.exp(8.0 + 1.5 * rng.standard_normal(n_bins)) / p[b]      # pool depth in token 1
+    recs, zp, R, g = [], [], [], []
+    for q in range(n_bins):
+        k = int(Ks[q])
+        if q < n_lb:                                   # Liquidity Book: bins around the active one
+            step = float(rng.choice([1, 2, 5, 10, 15, 20, 25, 50, 100])) * 1e-4
+            act = int(rng.integers(0, k))
+            off = np.arange(k) - act
+            prices = mid[q] * (1 + step) ** off
+            shape = np.exp(-0.5 * (off / max(k / 6, 1.0)) ** 2) if rng.random() < 0.7 else np.ones(k)
+            v = value[q] * shape / shape.sum()
+            x = np.where(off > 0, v / prices, 0.0); y = np.where(off < 0, v, 0.0)
+            share = rng.uniform(0.05, 0.95)
+            x[act], y[act] = share * v[act] / prices[act], (1 - share) * v[act]
+            fee = float(rng.choice([0.9999, 0.9995, 0.998]))
+        elif q < n_lb + n_book:                        # order book: k levels split between bids and asks
+            spread = rng.uniform(2e-4, 2e-3)
+            nb = int(rng.integers(0, k + 1)) if k > 1 else int(rng.integers(0, 2))
+            na = k - nb
+            tick = rng.uniform(1e-4, 1e-3)
+            bp_ = mid[q] * (1 - spread / 2) * (1 - tick) ** np.arange(nb)
+            ap_ = mid[q] * (1 + spread / 2) * (1 + tick) ** np.arange(na)
+            sz = value[q] / mid[q] * np.exp(rng.standard_normal(k)) / k
+            prices = np.concatenate([bp_[::-1], ap_])
+            x = np.concatenate([np.zeros(nb), sz[nb:]]); y = np.concatenate([bp_[::-1] * sz[:nb][::-1], np.zeros(na)])
+            fee = 1.0
+        else:                                          # one limit order, at up to 1 % through the mid
+            sell = rng.random() < 0.5
+            prices = np.array([mid[q] * (1 + (rng.uniform(-0.01, 0.01)))])
+            sz = value[q] / mid[q] * np.exp(rng.standard_normal()) * 0.1
+            x = np.array([sz if sell else 0.0]); y = np.array([0.0 if sell else prices[0] * sz])
+            fee = 1.0
+        r, z, pref, sums = bin_records(prices, x, y)
+        recs.append(r); zp.append((z, pref)); R += list(sums); g.append(fee)
+    m0 = m - n_bins
+    M = m
+    bin_ptr = np.zeros(M + 1, np.int64)
+    bin_ptr[m0 + 1:] = np.cumsum([len(r) for r in recs])
+    bin_zp = np.zeros((M, 2)); bin_zp[m0:] = np.asarray(zp).reshape(-1, 2)
+    hp = HostPools(n_tokens, np.arange(0, 2 * M + 1, 2, dtype=np.int64),
+                   np.concatenate([base["idx"].ravel(), np.stack([a, b], 1).ravel()]).astype(np.int32),
+                   np.concatenate([base["reserves"].ravel(), R]),
+                   np.concatenate([np.full(2 * m0, 0.5), np.zeros(2 * n_bins)]),
+                   np.concatenate([base["gamma"], g]),
+                   np.concatenate([np.full(m0, KIND_GEOMEAN_HOST), np.full(n_bins, KIND_BINS_HOST)]).astype(np.uint8),
+                   None, None, None, None, None, None, bin_ptr, np.concatenate(recs) if recs else None, bin_zp)
+    return hp, p

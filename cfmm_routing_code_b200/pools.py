@@ -25,9 +25,11 @@ ANN_MAX = 4e7           # largest StableSwap coefficient A n^n accepted, any coi
 STABLE_ARITY_MAX = 8    # most coins of a StableSwap pool
 KIND_CONCENTRATED_HOST = 6  # concentrated liquidity: a whole Uniswap-v3 tick ladder; records in HostPools.lad_rec
 KIND_CRYPTOSWAP_HOST = 8  # Curve cryptoswap, 2 or 3 coins; price scales ride in `weights`, A in HostPools.amp, gamma in .cgam
+KIND_BINS_HOST = 10     # price bins (Liquidity Book, order books, limit orders); records in HostPools.bin_rec
 CRYPTO_A_RANGE = (1e-6, 1e4)       # accepted whitepaper A of cryptoswap pools (the concavity of D is checked over it)
 CRYPTO_GAMMA_RANGE = (1e-6, 0.1)   # accepted curve gamma of cryptoswap pools (tests/test_cryptoswap.py checks the corners)
 LADDER_T_MAX = 1 << 20  # most intervals of one concentrated pool (cfmm_small::LADDER_T_MAX)
+BINS_K_MAX = 1 << 20    # most bins of one price-bin pool (cfmm_small::BINS_K_MAX)
 
 
 def ladder_records(bounds, liquidity) -> np.ndarray:
@@ -376,6 +378,72 @@ def _stable_groups(kind, pool_ptr):
     return [(int(k), ss[ar == k], ptr[ss[ar == k]][:, None] + np.arange(k)) for k in np.unique(ar).tolist()]
 
 
+def _check_bins(prices, x, y, where=""):
+    """The value rules of one price-bin pool given as (prices, x, y)"""
+    p, x, y = (np.asarray(v, np.float64).reshape(-1) for v in (prices, x, y))
+    if not (len(p) == len(x) == len(y)) or not 1 <= len(p) <= BINS_K_MAX:
+        raise ValueError(f"{where}bins need 1..{BINS_K_MAX} bins with one price, x and y each")
+    if not (np.all(np.isfinite(p) & (p > 0)) and np.all(np.diff(p) > 0)):
+        raise ValueError(f"{where}bin prices must be finite, > 0 and strictly increasing")
+    if not (np.all(np.isfinite(x) & (x >= 0)) and np.all(np.isfinite(y) & (y >= 0))) or not (x.any() or y.any()):
+        raise ValueError(f"{where}bin holdings must be finite, >= 0 and not all zero")
+    if x.any() and y.any() and p[y > 0].max() > p[x > 0].min():
+        raise ValueError(f"{where}bins are crossed: a bin holding token 1 prices above a bin holding token 0")
+    return p, x, y
+
+
+def bin_records(prices, x, y):
+    """Records of one price-bin pool (include/cfmm_b200.h, CFMM_KIND_BINS) from its checked (prices, x, y): (records
+    (nb, 4) {T, C, q, bin}, z, p_ref, (sum x, sum y)).  Both sides are summed outward from t = 0 in extended precision and
+    rounded once per record."""
+    p, x, y = (np.asarray(v, np.float64) for v in (prices, x, y))
+    ld = np.longdouble
+    bid = np.nonzero(y > 0)[0][::-1]                 # descending price: outward from t = 0
+    ask = np.nonzero(x > 0)[0]                       # ascending price
+    z, nb = len(bid), len(bid) + len(ask) + 1
+    rec = np.zeros((nb, 4))
+    rec[z + 1:, 0] = np.cumsum(x[ask].astype(ld)).astype(np.float64)
+    rec[z + 1:, 1] = np.cumsum(p[ask].astype(ld) * x[ask].astype(ld)).astype(np.float64)
+    rec[z:nb - 1, 2], rec[z:nb - 1, 3] = p[ask], ask
+    rec[:z, 0] = (-np.cumsum(y[bid].astype(ld) / p[bid].astype(ld))).astype(np.float64)[::-1]
+    rec[:z, 1] = (-np.cumsum(y[bid].astype(ld))).astype(np.float64)[::-1]
+    rec[:z, 2], rec[:z, 3] = p[bid][::-1], bid[::-1]
+    rec[nb - 1, 3] = -1.0
+    pref = float(p[ask[0]] if len(ask) else p[bid[0]])
+    sums = (float(np.sum(x.astype(ld))), float(np.sum(y.astype(ld))))
+    if not np.all(np.isfinite(rec)):
+        raise ValueError("bin records must be finite (token amounts out of fp64 range?)")
+    return rec, z, pref, sums
+
+
+def bin_fills(hp: "HostPools", i: int, t: float):
+    """How a net trade t of price-bin pool i (t > 0: the pool pays out t of token 0; t < 0: it takes in -t; the net-flow
+    form of CFMM_KIND_BINS) splits over its bins, best price first, at the bin prices and the pool's fee: (bins, flow0,
+    flow1), each bin's caller-order index and the token 0 and token 1 it pays to the trader (negative: it receives them,
+    tender before the fee).  The flows sum to (t, -C(t)) of the exact (eps = 0) evaluation; a t past the pool's depth is
+    filled up to its depth."""
+    if int(np.asarray(hp.kind)[i]) != KIND_BINS_HOST:
+        raise ValueError(f"pool {i} is not a bins pool")
+    rec = np.asarray(hp.bin_rec, np.float64).reshape(-1, 4)[int(hp.bin_ptr[i]):int(hp.bin_ptr[i + 1])]
+    z, g = int(hp.bin_zp[i, 0]), float(hp.gamma[i])
+    bins, f0, f1 = [], [], []
+    if t > 0:
+        for j in range(z, len(rec) - 1):
+            w = rec[j + 1, 0] - rec[j, 0]
+            f = min(w, t - rec[j, 0]) if rec[j + 1, 0] > t else w
+            bins.append(int(rec[j, 3])); f0.append(f); f1.append(-rec[j, 2] * f / g)
+            if rec[j + 1, 0] >= t:
+                break
+    elif t < 0:
+        for j in range(z - 1, -1, -1):
+            w = (rec[j + 1, 0] - rec[j, 0]) / g               # token 0 tendered (before the fee) to empty the bin
+            f = min(w, rec[j + 1, 0] / g - t)
+            bins.append(int(rec[j, 3])); f0.append(-f); f1.append(g * rec[j, 2] * f)
+            if rec[j, 0] / g <= t:
+                break
+    return np.asarray(bins, np.int64), np.asarray(f0), np.asarray(f1)
+
+
 @dataclasses.dataclass
 class HostPools:
     """CSR problem data on the host (numpy)."""
@@ -397,9 +465,20 @@ class HostPools:
     # cryptoswap pools (kind 8): the curve gamma G (the whitepaper A is in amp, the invariant D in inv, the price scales in
     # weights); 0 on other kinds.  None: all zero.
     cgam: Optional[np.ndarray] = None      # f64 [m]
+    # price-bin pools (kind 10): pool i's nb records are bin_rec[bin_ptr[i]:bin_ptr[i+1]] (none on other kinds), as
+    # bin_records; bin_zp[i] = (z, p_ref).  Their reserves are (sum x, sum y); their weights are 0.  None: no bins pools.
+    bin_ptr: Optional[np.ndarray] = None   # int64 [m+1]
+    bin_rec: Optional[np.ndarray] = None   # f64 [n_records, 4]
+    bin_zp: Optional[np.ndarray] = None    # f64 [m, 2]
 
     def __post_init__(self):
         m = len(self.gamma)
+        if self.bin_ptr is None:
+            self.bin_ptr = np.zeros(m + 1, np.int64)
+        if self.bin_rec is None:
+            self.bin_rec = np.zeros((0, 4))
+        if self.bin_zp is None:
+            self.bin_zp = np.zeros((m, 2))
         if self.lad_ptr is None:
             self.lad_ptr = np.zeros(m + 1, np.int64)
         if self.lad_rec is None:
@@ -439,7 +518,11 @@ class HostPools:
         curve's gamma (not the fee) and p_j the price scale times the precision of coin j (only p_0 / p_1 matters);
         A in CRYPTO_A_RANGE, G in CRYPTO_GAMMA_RANGE.  instances.twocrypto_pool converts a contract's state.  Three
         tokens (tricrypto-ng): weights[i] = (A, G, p_0, p_1, p_2), the same A and G rules, invariant tricrypto_invariant;
-        instances.tricrypto_pool converts a contract's state."""
+        instances.tricrypto_pool converts a contract's state.  And 'bins' (price bins: Liquidity Book bins, an order book,
+        limit orders): weights[i] = (prices, x, y) with the K bins' prices in token 1 per token 0 (the caller's units),
+        strictly increasing, and their holdings x of token 0 and y of token 1, finite, >= 0, not all 0, uncrossed (every
+        bin with y > 0 prices at or below every bin with x > 0), 1 <= K <= BINS_K_MAX; reserves[i] must be None (they are
+        (sum x, sum y)).  instances.lb_bins and instances.order_book build the triple."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
@@ -447,8 +530,20 @@ class HostPools:
         amp = np.zeros(m)
         cgam = np.zeros(m)
         lad = {}                                         # concentrated pool -> its records and price
+        bins = {}                                        # bins pool -> bin_records
         for i, l in enumerate(local_indices):
             k = len(l)
+            if kinds[i] == "bins":
+                if k != 2 or len(set(int(t) for t in l)) != 2:
+                    raise ValueError(f"pool {i}: bins pools need 2 distinct tokens")
+                if reserves[i] is not None:
+                    raise ValueError(f"pool {i}: a bins pool's reserves[i] must be None (they are derived)")
+                if weights is None or weights[i] is None or len(weights[i]) != 3:
+                    raise ValueError(f"pool {i}: bins needs weights[i] = (prices, x, y)")
+                bins[i] = bin_records(*_check_bins(*weights[i], where=f"pool {i}: "))
+                ptr.append(ptr[-1] + 2); idx += [int(t) for t in l]; res += list(bins[i][3]); wts += [0.0, 0.0]
+                kd.append(KIND_BINS_HOST)
+                continue
             if kinds[i] == "concentrated":
                 if k != 2 or len(set(int(t) for t in l)) != 2:
                     raise ValueError(f"pool {i}: concentrated pools need 2 distinct tokens")
@@ -514,10 +609,17 @@ class HostPools:
             lad_sc[ids, 0], lad_sc[ids, 1] = sv, cv
             first = np.asarray(ptr, np.int64)[ids]
             res[first], res[first + 1] = x, y
+        bin_ptr = np.zeros(m + 1, np.int64); bin_zp = np.zeros((m, 2)); brec = None
+        if bins:
+            cnt = np.zeros(m, np.int64)
+            for i, b in bins.items():
+                cnt[i] = len(b[0]); bin_zp[i] = (b[1], b[2])
+            bin_ptr[1:] = np.cumsum(cnt)
+            brec = np.concatenate([bins[i][0] for i in sorted(bins)])
         return HostPools(int(n_tokens), np.asarray(ptr, np.int64), np.asarray(idx, np.int32),
                          res, np.asarray(wts, np.float64),
                          np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp, None, lad_ptr,
-                         np.concatenate(recs) if recs else None, lad_sc, cgam)
+                         np.concatenate(recs) if recs else None, lad_sc, cgam, bin_ptr, brec, bin_zp)
 
     @staticmethod
     def from_pairs(n_tokens, idx, reserves, gamma) -> "HostPools":
@@ -542,14 +644,16 @@ class HostPools:
 
     def validate(self):
         slot_kind = np.repeat(np.asarray(self.kind), np.diff(self.pool_ptr)) if \
-            np.any((self.kind == KIND_BOUNDED_HOST) | (self.kind == KIND_CONCENTRATED_HOST)) else None
+            np.any((self.kind == KIND_BOUNDED_HOST) | (self.kind == KIND_CONCENTRATED_HOST) | (self.kind == KIND_BINS_HOST)) \
+            else None
         virt = self.reserves if slot_kind is None else self.reserves + np.where(slot_kind == KIND_BOUNDED_HOST, self.weights, 0.0)
         lo_ok = np.all(self.reserves > 0) if slot_kind is None else np.all(self.reserves >= 0) and \
-            np.all((virt > 0) | (slot_kind == KIND_CONCENTRATED_HOST))
+            np.all((virt > 0) | (slot_kind == KIND_CONCENTRATED_HOST) | (slot_kind == KIND_BINS_HOST))
         if not lo_ok or not np.all(np.isfinite(self.reserves)):
             raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves; "
-                             "concentrated: >= 0)")
+                             "concentrated, bins: >= 0)")
         self._validate_ladders()
+        self._validate_bins()
         if np.any(self.gamma <= 0) or np.any(self.gamma > 1):
             raise ValueError("fees (gamma) must lie in (0, 1]")
         if self.tok_idx.min(initial=0) < 0 or self.tok_idx.max(initial=0) >= self.n_tokens:
@@ -569,6 +673,34 @@ class HostPools:
             if not bool(np.all(np.isfinite(D) & (D > 0))):
                 raise ValueError("cryptoswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
 
+
+    def _validate_bins(self):
+        """The rules of price-bin pools on the CSR form: arity 2; 2 .. BINS_K_MAX + 2 records, none on other kinds; T
+        strictly increasing and finite, record z = (0, 0), C finite, segment prices finite and > 0, p_ref finite, > 0."""
+        kind, m = np.asarray(self.kind), self.m
+        ptr = np.asarray(self.bin_ptr, np.int64)
+        rec = np.asarray(self.bin_rec, np.float64).reshape(-1, 4)
+        if len(ptr) != m + 1 or ptr[0] != 0 or np.any(np.diff(ptr) < 0) or ptr[-1] != len(rec):
+            raise ValueError("bin_ptr must be a CSR pointer of m + 1 entries over bin_rec")
+        bn = kind == KIND_BINS_HOST
+        cnt = np.diff(ptr)
+        if np.any(cnt[~bn] != 0) or np.any((cnt[bn] < 2) | (cnt[bn] > BINS_K_MAX + 2)):
+            raise ValueError(f"bins pools need 1..{BINS_K_MAX} bins (2 .. {BINS_K_MAX + 2} records); other kinds none")
+        if not bn.any():
+            return
+        ids = np.nonzero(bn)[0]
+        if np.any(np.diff(self.pool_ptr)[ids] != 2):
+            raise ValueError("bins pools must have 2 tokens")
+        owner = np.repeat(np.arange(m), cnt)
+        last = np.zeros(len(rec), bool); last[ptr[ids + 1] - 1] = True
+        inc = np.ones(len(rec), bool); inc[1:] = (rec[1:, 0] > rec[:-1, 0]) | (owner[1:] != owner[:-1])
+        if not (np.all(np.isfinite(rec)) and np.all(inc) and np.all((rec[~last, 2] > 0))):
+            raise ValueError("bin records must be finite, T strictly increasing, segment prices > 0")
+        z, pref = np.asarray(self.bin_zp, float)[ids, 0], np.asarray(self.bin_zp, float)[ids, 1]
+        ok = (z == np.floor(z)) & (z >= 0) & (z < cnt[ids]) & np.isfinite(pref) & (pref > 0)
+        zi = ptr[ids] + np.where(ok, z, 0).astype(np.int64)
+        if not bool(np.all(ok & (rec[zi, 0] == 0) & (rec[zi, 1] == 0))):
+            raise ValueError("bins (z, p_ref): record z must be the t = 0 breakpoint and p_ref finite and > 0")
 
     def _validate_ladders(self):
         """The rules of concentrated pools on the CSR form: arity 2; T + 1 records, 1 <= T <= LADDER_T_MAX, none on other
@@ -690,6 +822,8 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
         raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates, curve_gamma or several")
     if n and (ids.min() < 0 or ids.max() >= m):
         raise ValueError(f"pool id out of range [0, {m})")
+    if reserves is not None and bool(np.any(np.asarray(kind)[ids] == KIND_BINS_HOST)):
+        raise ValueError("bins pools take no reserves= (their reserves are derived from the bins, which are structure)")
     conc = np.asarray(kind)[ids] == KIND_CONCENTRATED_HOST
     if reserves is not None and conc.any():
         raise ValueError("concentrated pools take prices=, not reserves= (their reserves are derived from the price)")
@@ -862,6 +996,11 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         if np.any(ar[cl] != 2):
             raise ValueError("concentrated pools must have 2 tokens")
         keys.append((_lib.KIND_CONCENTRATED, 2, np.nonzero(cl)[0]))
+    bn = hp.kind == KIND_BINS_HOST
+    if bn.any():
+        if np.any(ar[bn] != 2):
+            raise ValueError("bins pools must have 2 tokens")
+        keys.append((_lib.KIND_BINS, 2, np.nonzero(bn)[0]))
     cs = hp.kind == KIND_CRYPTOSWAP_HOST
     if cs.any():
         if np.any((ar[cs] != 2) & (ar[cs] != 3)):
@@ -944,7 +1083,17 @@ class DeviceBucket:
             sc = np.asarray(hp.lad_sc, np.float64)[sel]
             P = np.stack([sc[:, 0], sc[:, 1], loc.astype(np.float64), (cnt - 1).astype(np.float64)])
             self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
-        if self.kind == _lib.KIND_SUM:
+        if self.kind == _lib.KIND_BINS:                    # records in the weights slot, (first, nb, z, p_ref) in logrw
+            sel = spec.sel
+            first = np.asarray(hp.bin_ptr, np.int64)[sel]
+            cnt = np.asarray(hp.bin_ptr, np.int64)[sel + 1] - first
+            loc = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
+            gather = np.repeat(first - loc, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
+            self.weights = torch.as_tensor(np.ascontiguousarray(np.asarray(hp.bin_rec, np.float64)[gather]).reshape(-1), **f64)
+            zp = np.asarray(hp.bin_zp, np.float64)[sel]
+            P = np.stack([loc.astype(np.float64), cnt.astype(np.float64), zp[:, 0], zp[:, 1]])
+            self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
+        if self.kind in (_lib.KIND_SUM, _lib.KIND_BINS):
             self.theta_bar = torch.zeros((2, self.stride), **f64)
         self.delta = self.lam = self.hcoef = self.hmask = None
         self._device = device
@@ -1491,7 +1640,7 @@ class PoolStore:
         self._blocked_first = bool(self.buckets) and getattr(self.buckets[0], "blocked", False)
         assert sum(1 for b in self.buckets if getattr(b, "blocked", False)) <= 1
         self.m_local = sum(b.m for b in self.buckets)
-        self.has_sum = bool(np.any(hp.kind == KIND_SUM_HOST))
+        self.has_sum = bool(np.any((hp.kind == KIND_SUM_HOST) | (hp.kind == KIND_BINS_HOST)))
         self.has_geomean = any(b.kind == _lib.KIND_GEOMEAN for b in self.buckets)
         f64 = dict(dtype=torch.float64, device=self.device)
         # [psi | arb] (the one all-reduced buffer) and y are ping-ponged: a blocked launch clears the buffer of the
@@ -1631,6 +1780,10 @@ class PoolStore:
                 _lib.check(self.lib.cfmm_sum_update_multipliers(C.byref(b.c_bucket), b.lam.data_ptr(),
                                                                 b.theta_bar.data_ptr(), self._move.data_ptr(), st),
                            "cfmm_sum_update_multipliers")
+            elif b.kind == _lib.KIND_BINS:
+                _lib.check(self.lib.cfmm_bins_update_multipliers(C.byref(b.c_bucket), b.delta.data_ptr(), b.lam.data_ptr(),
+                                                                 b.theta_bar.data_ptr(), self._move.data_ptr(), st),
+                           "cfmm_bins_update_multipliers")
         return self._move
 
     def reset_multipliers(self):

@@ -77,7 +77,31 @@ enum {
                               edge weights (w01, w02, w12) of the pool's scaled Hessian block, Hs = sum_{a<b} w_ab
                               (e_a - e_b)(e_a - e_b)' (Hs 1 = 0; one weight may be negative, Hs is PSD), 0 on an edge
                               with an untraded end; hmask = the traded slots (required by the HVP, diagonal and dense
-                              kernels).  Smooth: no theta_bar                                                        */
+                              kernels).  Smooth: no theta_bar                                                        */,
+    CFMM_KIND_BINS = 10       /* price bins (Liquidity Book bins, an order book, limit orders): bins k at prices p_k (token
+                              1 per token 0) holding x_k >= 0 of token 0 and y_k >= 0 of token 1, uncrossed (every bin
+                              with y > 0 prices at or below every bin with x > 0); bin k accepts (D, L) iff
+                              p_k (x_k + gamma D_0 - L_0) + (y_k + gamma D_1 - L_1) >= p_k x_k + y_k and both new
+                              holdings are >= 0, and the trading set is the Minkowski sum of the bins'.  Not in the
+                              reference; arity 2.  In net-flow form the pool pays out t of token 0 for the least C(t) of
+                              token 1, C convex piecewise linear on [-S_bid, S_ask] (asks: slope p_k / gamma over x_k;
+                              bids: slope gamma p_k over y_k / (gamma p_k)).  weights = the records, AoS, 4 f64 per
+                              breakpoint {T_j, C_j, q_j, bin}, ascending in T, fee-free: record z is (0, 0); above it T
+                              is the cumulative x and C the cumulative p x of the asks, below it T is minus the
+                              cumulative y / p and C minus the cumulative y of the bids, both accumulated outward from
+                              t = 0; q_j = the price of segment (j, j+1) and bin its caller-order bin index (0 and -1 on
+                              the last record).  The kernel applies the fee: T / gamma below z, C / gamma above it.  A
+                              pool's nb records are consecutive.  logrw [4][stride]: slot 0 = the index of its first
+                              record in `weights`, slot 1 = nb (2 .. 2^20 + 2), slot 2 = z (in the pool's records),
+                              slot 3 = p_ref > 0 (a fixed price of the pool: the ask price at t = 0, else the bid
+                              price).  reserves [2][stride] = (sum x, sum y) (not read by the evaluation).  eps = 0:
+                              t maximises r t - C(t), r = nu0 / nu1, a segment filling only when strictly profitable.
+                              eps > 0: t maximises r t - C(t) - p_ref (t - tbar)^2 / (2 sigma), sigma = S / eps, S =
+                              S_bid + S_ask, with tbar = theta_bar row 0 (row 1 unused; required), and the trader
+                              pays the smoothing term.  delta / lambda: the positive and negative parts of the flows
+                              (t, -(C(t) + smoothing)).  hcoef per pool, as for every pair kind: (sigma / p_ref) r nu0
+                              inside a segment, 0 at a breakpoint or an end.  cfmm_bins_update_multipliers advances
+                              tbar.                                                                                    */
 };
 
 enum {
@@ -99,9 +123,10 @@ typedef struct cfmm_bucket {
     const double* reserves;
     const int32_t* tok_idx;
     const double* gamma;
-    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates; CONCENTRATED records */
-    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D); CONCENTRATED (s, c, first record, T) */
-    const double* theta_bar; /* SUM only     */
+    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates; CONCENTRATED, BINS records */
+    const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D); CONCENTRATED (s, c, first record, T);
+                                BINS (first record, nb, z, p_ref) */
+    const double* theta_bar; /* SUM and BINS only */
 } cfmm_bucket;
 
 /* Optional per-pool outputs of one evaluation (any pointer may be NULL). */
@@ -315,7 +340,8 @@ int cfmm_blocked_solve_peer(const cfmm_blocked_pairs* b, int32_t n_tokens, const
  * this loop the steepest-descent one.  cfmm_blocked_solve is this loop's one-blocked-bucket case.
  * outs[k]: bucket k's per-pool outputs, used as cfmm_arb_eval's `out`.  Every non-empty bucket needs hcoef, and hmask
  * for GEOMEAN, STABLESWAP_N and CRYPTOSWAP_3 (CFMM_E_NULL otherwise); delta / lambda receive the trades of the final
- * read-back (may be NULL, except lambda of a SUM bucket, whose theta_bar the loop resets and advances: CFMM_E_NULL).
+ * read-back (may be NULL, except lambda of a SUM bucket and both of a BINS bucket, whose theta_bar the loop resets and
+ * advances: CFMM_E_NULL).
  * blocked_out: the blocked bucket's delta / lambda (blocked order), or NULL; its hcoef lives in `work`.
  * Utility, c / a / eq / pinned / nu / psi_out and res as for cfmm_blocked_solve; `work`:
  * cfmm_market_solve_work_bytes() bytes (same buckets, blocked, n_tokens and linear_solver).  Allocates no device memory;
@@ -389,7 +415,7 @@ typedef struct cfmm_csr_pools {
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
     const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP |
                                             CFMM_KIND_CONCENTRATED | CFMM_KIND_CRYPTOSWAP |
-                                            CFMM_KIND_CRYPTOSWAP_3, else weighted
+                                            CFMM_KIND_CRYPTOSWAP_3 | CFMM_KIND_BINS, else weighted
                                             geometric mean                                           */
 } cfmm_csr_pools;
 
@@ -450,6 +476,14 @@ int cfmm_batch_solve_cryptoswap(const cfmm_csr_pools* pools, const double* recor
  * others keep their registers.  Same limits and workspace. */
 int cfmm_batch_solve_tricrypto(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
                                const cfmm_batch_params* prm, void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_BINS pools, beside every kind cfmm_batch_solve_tricrypto takes (the
+ * six entry points above give their problems status 3).  In the CSR arrays a bins pool carries z and p_ref in its two
+ * weights slots, its first record and nb in its two logrw slots, and (sum x, sum y) in its reserves; records: the
+ * concentrated and bins pools' records in one buffer (CFMM_E_NULL if NULL).  The multiplier tbar lives in the pool's
+ * first theta_bar slot of the workspace.  A seventh kernel instance, so the others keep their registers.  Same limits
+ * and workspace. */
+int cfmm_batch_solve_bins(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
+                          const cfmm_batch_params* prm, void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
@@ -466,6 +500,12 @@ int cfmm_allreduce_ll(const double* local, const void* peer_recv_dev, int32_t ra
 /* SUM buckets: theta_bar <- current fills (= lambda), returns max_i |change|/R in move[0] (device). */
 int cfmm_sum_update_multipliers(const cfmm_bucket* bucket, const double* lambda, double* theta_bar_out,
                                 double* move, void* stream);
+
+/* BINS buckets: theta_bar row 0 (tbar) <- t = lambda_0 - delta_0, the net token-0 flows of the last trades evaluation
+ * (delta, lambda [2][stride]); returns max_i |change| / S_i in move[0] (device; the caller zeroes it first), S_i the
+ * width of pool i's net-flow domain at its fee.  CFMM_E_KIND unless kind BINS, arity 2. */
+int cfmm_bins_update_multipliers(const cfmm_bucket* bucket, const double* delta, const double* lambda,
+                                 double* theta_bar_out, double* move, void* stream);
 
 /* cudaMemsetAsync(ptr, 0, bytes) on the stream -- lets a host language zero psi/arb without torch. */
 int cfmm_zero(void* ptr, int64_t bytes, void* stream);
