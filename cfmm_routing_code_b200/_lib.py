@@ -134,6 +134,8 @@ def load(build_if_missing: bool = True):
     lib.cfmm_ladder_splice_work_bytes.restype = i64
     lib.cfmm_ladder_splice.argtypes = [C.POINTER(Bucket), i64, vp, vp, vp, i64, vp, vp, i64, C.POINTER(i64), vp, i64, vp]
     lib.cfmm_ladder_splice.restype = C.c_int
+    lib.cfmm_bins_splice.argtypes = [C.POINTER(Bucket), i64, vp, vp, vp, i64, vp, vp, i64, C.POINTER(i64), vp, i64, vp]
+    lib.cfmm_bins_splice.restype = C.c_int
     lib.cfmm_blocked_eval.argtypes = [C.POINTER(BlockedPairs), i32, vp, vp, vp, C.POINTER(EvalOut), vp, i64, vp]
     lib.cfmm_blocked_eval.restype = C.c_int
     lib.cfmm_blocked_hvp.argtypes = [C.POINTER(BlockedPairs), i32, vp, vp, vp, vp, vp]

@@ -724,3 +724,52 @@ def synth_bins_market(m, n_tokens, seed, K=(1, 256), frac_lb=0.3, frac_book=0.1,
                    np.concatenate([np.full(m0, KIND_GEOMEAN_HOST), np.full(n_bins, KIND_BINS_HOST)]).astype(np.uint8),
                    None, None, None, None, None, None, bin_ptr, np.concatenate(recs) if recs else None, bin_zp)
     return hp, p
+
+
+def bins_event(rng, triple, what=None, k_max=256):
+    """One block's change of a price-bin pool given as its (prices, x, y), as the new triple (the rules of
+    HostPools.from_lists hold for it): what = 'swap' (a Liquidity Book swap empties the active bin and moves it one to
+    three bins: the top bids turn into asks at their prices, or the bottom asks into bids), 'deposit' (one to four bins
+    added past an end, K grows up to k_max), 'withdraw' (one to four bins at an end removed, K shrinks, at least one
+    bin with holdings stays), 'book' (order-book levels change: the mid moves through one to four ask or bid levels, which
+    are taken and reposted on the other side at the same prices, a new level appears past the far end, and every size
+    moves by a few percent) or 'fill' (a partial fill of the one-bin limit order: a share of its holding turns into the
+    other token at its price; another pool gets a swap); None: one drawn at random."""
+    p, x, y = (np.asarray(v, np.float64).reshape(-1).copy() for v in triple)
+    what = what or rng.choice(["swap", "deposit", "withdraw", "book", "fill"])
+    K = len(p)
+    if what == "fill" and K == 1:
+        f = rng.uniform(0.1, 0.9)
+        if x[0] > 0:
+            x[0], y[0] = x[0] * (1 - f), y[0] + p[0] * x[0] * f
+        else:
+            y[0], x[0] = y[0] * (1 - f), x[0] + y[0] / p[0] * f
+        return p, x, y
+    if what in ("swap", "fill", "book"):
+        s = int(rng.integers(1, 4 if what != "book" else 5))
+        down = (rng.random() < 0.5 and y.any()) or not x.any()
+        if down:                                       # token 0 sold into the pool: the top bids become asks
+            j = np.nonzero(y > 0)[0][::-1][:s]
+            x[j] += y[j] / p[j]; y[j] = 0.0
+        else:                                          # token 0 bought from the pool: the bottom asks become bids
+            j = np.nonzero(x > 0)[0][:s]
+            y[j] += x[j] * p[j]; x[j] = 0.0
+        if what != "book":
+            return p, x, y
+        x *= np.exp(0.05 * rng.standard_normal(K)); y *= np.exp(0.05 * rng.standard_normal(K))
+        what = "deposit"                               # and a new level past the far end
+    step = float(np.exp(np.mean(np.log(p[1:] / p[:-1])))) if K > 1 else 1.001
+    if what == "deposit" and K < k_max:
+        n = int(min(rng.integers(1, 5), k_max - K))
+        v = float(np.sum(x * p + y)) / max(K, 1)
+        if rng.random() < 0.5:                         # new asks above
+            q = p[-1] * step ** np.arange(1, n + 1)
+            return np.r_[p, q], np.r_[x, v / q], np.r_[y, np.zeros(n)]
+        q = p[0] * step ** -np.arange(n, 0, -1)         # new bids below
+        return np.r_[q, p], np.r_[np.zeros(n), x], np.r_[np.full(n, v), y]
+    if K > 1:                                          # withdraw (or a deposit past k_max): bins at one end go
+        n = int(min(rng.integers(1, 5), K - 1))
+        keep = slice(n, K) if rng.random() < 0.5 else slice(0, K - n)
+        if (x[keep] > 0).any() or (y[keep] > 0).any():
+            return p[keep], x[keep], y[keep]
+    return p, x, y

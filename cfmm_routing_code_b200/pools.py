@@ -126,9 +126,10 @@ def new_ladders(ladders):
 
 
 class LadderSlab:
-    """The host records of a store's concentrated pools, replaceable pool by pool (PoolStore.update_pools(ladders=)).
-    Pool i's T[i] + 1 records start at first[i] of the concatenation [base | own] (T[i] = -1: not a ladder): `base` is
-    a HostPools' lad_rec, borrowed and never written, `own` an append-only slab of the ladders that replaced others.  A
+    """The host records of a store's concentrated pools (or of its price-bin pools), replaceable pool by pool
+    (PoolStore.update_pools(ladders=), (bins=)).  Pool i's T[i] + 1 records start at first[i] of the concatenation
+    [base | own] (T[i] = -1: no records; a bins pool's T is nb - 1): `base` is a HostPools' lad_rec (bin_rec), borrowed
+    and never written, `own` an append-only slab of the record runs that replaced others.  A
     replacement appends its records and leaves the ones it supersedes dead; once the dead records outnumber the live
     ones, the live ones are compacted into a new slab in pool order and the base is let go.  So one replacement costs
     O(its records) plus O(m) integer work, amortised, not a copy of every record."""
@@ -416,6 +417,21 @@ def bin_records(prices, x, y):
     return rec, z, pref, sums
 
 
+def new_bins(triples):
+    """Records and state of price-bin pools given as (prices, x, y) triples (already checked), each as
+    HostPools.from_lists makes them: bin_records of the pool alone.  Returns (records (sum nb, 4) pool after pool,
+    counts nb (n,) int64, state (n, 4) f64 = (z, p_ref, sum x, sum y)), the arguments of cfmm_bins_splice."""
+    return _pack_bins([bin_records(*t) for t in triples])
+
+
+def _pack_bins(recs):
+    """new_bins from the pools' bin_records results"""
+    cnt = np.asarray([len(r[0]) for r in recs], np.int64)
+    rec = np.concatenate([r[0] for r in recs]) if recs else np.zeros((0, 4))
+    state = np.asarray([(r[1], r[2], r[3][0], r[3][1]) for r in recs], np.float64).reshape(-1, 4)
+    return rec, cnt, state
+
+
 def bin_fills(hp: "HostPools", i: int, t: float):
     """How a net trade t of price-bin pool i (t > 0: the pool pays out t of token 0; t < 0: it takes in -t; the net-flow
     form of CFMM_KIND_BINS) splits over its bins, best price first, at the bin prices and the pool's fee: (bins, flow0,
@@ -425,7 +441,11 @@ def bin_fills(hp: "HostPools", i: int, t: float):
     if int(np.asarray(hp.kind)[i]) != KIND_BINS_HOST:
         raise ValueError(f"pool {i} is not a bins pool")
     rec = np.asarray(hp.bin_rec, np.float64).reshape(-1, 4)[int(hp.bin_ptr[i]):int(hp.bin_ptr[i + 1])]
-    z, g = int(hp.bin_zp[i, 0]), float(hp.gamma[i])
+    return _bin_fills(rec, int(hp.bin_zp[i, 0]), float(hp.gamma[i]), t)
+
+
+def _bin_fills(rec, z, g, t):
+    """bin_fills of one pool given by its records (nb, 4), the index z of its t = 0 record and its fee g"""
     bins, f0, f1 = [], [], []
     if t > 0:
         for j in range(z, len(rec) - 1):
@@ -782,6 +802,7 @@ class PoolUpdate:
     amp: Optional[np.ndarray] = None      # f64 [n] new amplifications A of StableSwap pools, or None
     rates: Optional[np.ndarray] = None    # f64 [nnz] new rates (price scales) of StableSwap (cryptoswap) pools at `slots`
     curve_gamma: Optional[np.ndarray] = None   # f64 [n] new curve gammas of cryptoswap pools, or None
+    bins: Optional[list] = None           # [n] bin_records of the new (prices, x, y) of price-bin pools, or None
 
 
 def _pool_rows(vals, n, ar, what):
@@ -799,7 +820,8 @@ def _pool_rows(vals, n, ar, what):
 
 
 def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarray, pool_ids, reserves=None,
-                      fees=None, prices=None, ladders=None, amp=None, rates=None, curve_gamma=None) -> PoolUpdate:
+                      fees=None, prices=None, ladders=None, amp=None, rates=None, curve_gamma=None,
+                      bins=None) -> PoolUpdate:
     """Host checks of PoolStore.update_pools, on the problem's CSR arrays (pool_ptr, kind, weights as in HostPools).
     pool_ids: global pool indices, distinct and in range; reserves[k]: the new reserve vector of pool pool_ids[k] with the
     pool's arity (a row of the reference's `reserves` literal; an (n, k) array when all pools have arity k); fees[k]: its
@@ -810,16 +832,20 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
     from_lists); not together with prices=.  amp[k]: the new whitepaper A of StableSwap pool pool_ids[k], rates[k]: its new
     rate vector (the pool's arity; an (n, k) array as for reserves), under the rules of from_lists.  For cryptoswap pools
     amp[k] is the new whitepaper A, rates[k] the new price scales (p_0, p_1[, p_2]), curve_gamma[k] the new curve gamma (cryptoswap
-    pools only); amp= and rates= may not mix StableSwap and cryptoswap pools in one call.
-    Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order."""
+    pools only); amp= and rates= may not mix StableSwap and cryptoswap pools in one call.  bins[k]: the new
+    (prices, x, y) of price-bin pool pool_ids[k], the triple of HostPools.from_lists' weights[i] (K may differ from the
+    pool's old K; the rules of from_lists, and records finite as bin_records checks); a bins pool takes no reserves=.
+    Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order and the
+    new bins as their bin_records."""
     m = len(pool_ptr) - 1
     ids = np.asarray(pool_ids)
     if ids.ndim != 1 or (ids.size and not np.issubdtype(ids.dtype, np.integer)):
         raise ValueError("pool_ids must be a 1-d sequence of integer pool indices")
     ids = ids.astype(np.int64)
     n = len(ids)
-    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates, curve_gamma)):
-        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates, curve_gamma or several")
+    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates, curve_gamma, bins)):
+        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates, curve_gamma, bins or "
+                         "several")
     if n and (ids.min() < 0 or ids.max() >= m):
         raise ValueError(f"pool id out of range [0, {m})")
     if reserves is not None and bool(np.any(np.asarray(kind)[ids] == KIND_BINS_HOST)):
@@ -880,6 +906,21 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             _check_ladder(t[0], t[1], t[2], f"ladders[{k}]: ")
             lad.append((float(np.asarray(t[0], np.float64).reshape(-1)[0]), np.asarray(t[1], np.float64).reshape(-1),
                         np.asarray(t[2], np.float64).reshape(-1)))
+    brec = None
+    if bins is not None:
+        if len(bins) != n:
+            raise ValueError("bins: one (prices, x, y) per pool")
+        if not bool(np.all(np.asarray(kind)[ids] == KIND_BINS_HOST)):
+            raise ValueError("bins= applies to bins pools only")
+        brec = []
+        for k, t in enumerate(bins):
+            if t is None or len(t) != 3:
+                raise ValueError(f"bins[{k}]: bins needs (prices, x, y)")
+            checked = _check_bins(*t, where=f"bins[{k}]: ")
+            try:
+                brec.append(bin_records(*checked))
+            except ValueError as e:
+                raise ValueError(f"bins[{k}]: {e}") from None
     A = W = CG = None
     crypto = np.asarray(kind)[ids] == KIND_CRYPTOSWAP_HOST
     if curve_gamma is not None:
@@ -912,7 +953,7 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             _check_stableswap(np.ones(len(sel)) if A is None else A[sel],
                               np.ones((len(sel), k)) if W is None else W[first[sel][:, None] + np.arange(k)],
                               np.ones((len(sel), k)))
-    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W, CG)
+    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W, CG, brec)
 
 
 class BucketSpec:
@@ -1079,7 +1120,7 @@ class DeviceBucket:
             gather = np.repeat(first - loc, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
             self.weights = torch.as_tensor(np.ascontiguousarray(np.asarray(hp.lad_rec, np.float64)[gather]).reshape(-1), **f64)
             self.n_rec = int(cnt.sum())
-            self._rec_buf, self._rec_spare = self.weights, None      # splice_ladders writes the spare and swaps
+            self._rec_buf, self._rec_spare = self.weights, None      # splice_records writes the spare and swaps
             sc = np.asarray(hp.lad_sc, np.float64)[sel]
             P = np.stack([sc[:, 0], sc[:, 1], loc.astype(np.float64), (cnt - 1).astype(np.float64)])
             self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
@@ -1090,6 +1131,8 @@ class DeviceBucket:
             loc = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
             gather = np.repeat(first - loc, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)
             self.weights = torch.as_tensor(np.ascontiguousarray(np.asarray(hp.bin_rec, np.float64)[gather]).reshape(-1), **f64)
+            self.n_rec = int(cnt.sum())
+            self._rec_buf, self._rec_spare = self.weights, None      # as for concentrated buckets
             zp = np.asarray(hp.bin_zp, np.float64)[sel]
             P = np.stack([loc.astype(np.float64), cnt.astype(np.float64), zp[:, 0], zp[:, 1]])
             self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
@@ -1143,12 +1186,15 @@ class DeviceBucket:
         if gamma is not None:
             self.gamma[li] = torch.as_tensor(gamma, **f64)
 
-    def splice_ladders(self, lib, loc: np.ndarray, rec: np.ndarray, cnt: np.ndarray, state: np.ndarray, n_total: int,
+    def splice_records(self, lib, loc: np.ndarray, rec: np.ndarray, cnt: np.ndarray, state: np.ndarray, n_total: int,
                        stream):
-        """New ladders of the concentrated pools at the bucket-local positions `loc` (ascending): their records rec
-        (sum(cnt), 4), pool after pool, cnt[k] = T + 1 of pool loc[k], state (n, 4) = (s, c, x, y).  cfmm_ladder_splice
-        writes every pool's records into the spare buffer in bucket order (n_total of them), then the two buffers swap, so
-        c_bucket.weights moves (a CUDA graph captured over this bucket must be captured again).  Synchronous."""
+        """New records of the pools at the bucket-local positions `loc` (ascending): rec (sum(cnt), 4), pool after pool.
+        Concentrated buckets (cfmm_ladder_splice): cnt[k] = T + 1 of pool loc[k], state (n, 4) = (s, c, x, y).  Price-bin
+        buckets (cfmm_bins_splice): cnt[k] = nb, state = (z, p_ref, sum x, sum y), and the changed pools' theta_bar is
+        zeroed (a fresh pool's multiplier).  The entry point writes every pool's records into the spare buffer in bucket
+        order (n_total of them), then the two buffers swap, so c_bucket.weights moves (a CUDA graph captured over this
+        bucket must be captured again).  Synchronous."""
+        name = "cfmm_bins_splice" if self.kind == _lib.KIND_BINS else "cfmm_ladder_splice"
         dev = self._device
         if self._rec_spare is None or self._rec_spare.numel() < 4 * n_total:
             self._rec_spare = None
@@ -1163,13 +1209,14 @@ class DeviceBucket:
             _lib.check(nb, "cfmm_ladder_splice_work_bytes")
         work = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
         status = (C.c_int64 * 2)()
-        _lib.check(lib.cfmm_ladder_splice(C.byref(self.c_bucket), len(loc), pos.data_ptr(), nrec.data_ptr(),
-                                          recd.data_ptr(), len(rec), std.data_ptr(), self._rec_spare.data_ptr(),
-                                          self._rec_spare.numel() // 4, status, work.data_ptr(), nb, stream),
-                   "cfmm_ladder_splice")
+        _lib.check(getattr(lib, name)(C.byref(self.c_bucket), len(loc), pos.data_ptr(), nrec.data_ptr(),
+                                      recd.data_ptr(), len(rec), std.data_ptr(), self._rec_spare.data_ptr(),
+                                      self._rec_spare.numel() // 4, status, work.data_ptr(), nb, stream), name)
         if status[0] != 0 or status[1] != n_total:
-            raise _lib.CfmmError(f"cfmm_ladder_splice rejected the update ({status[0]} invalid entries, {status[1]} records "
+            raise _lib.CfmmError(f"{name} rejected the update ({status[0]} invalid entries, {status[1]} records "
                                  f"for {n_total} expected)")
+        if self.theta_bar is not None and len(loc):
+            self.theta_bar[:, pos] = 0.0
         self._rec_buf, self._rec_spare = self._rec_spare, self._rec_buf
         self.weights = self._rec_buf[:4 * n_total]
         self.n_rec = n_total
@@ -1623,6 +1670,8 @@ class PoolStore:
         self._own_stable = False                                         # weights / amp are this store's copies
         self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records
         self._lad = None                                                 # LadderSlab
+        self._bins_host = (hp.bin_ptr, hp.bin_rec)                       # price-bin records
+        self._bin = None                                                 # LadderSlab of the price-bin records
         self._where = None                                               # pool -> (bucket, position): update_pools
         self.rank, self.world = rank, world
         self.buckets = []
@@ -1822,9 +1871,28 @@ class PoolStore:
             self._lad = LadderSlab(*self._lad_host)
         return self._lad
 
+    def _bins(self) -> LadderSlab:
+        if self._bin is None:
+            self._bin = LadderSlab(*self._bins_host)
+        return self._bin
+
+    def bin_fills(self, i: int, t: float):
+        """pools.bin_fills of price-bin pool i as this store holds it now: its current bins (after update_pools(bins=);
+        the caller's HostPools still describes the old ones) and its current fee, read from the device.  ValueError if
+        pool i is not a bins pool or is held by another rank."""
+        i = int(i)
+        if not 0 <= i < self.m_total or int(np.asarray(self._kind_host)[i]) != KIND_BINS_HOST:
+            raise ValueError(f"pool {i} is not a bins pool")
+        bi, loc = self._pool_map()
+        if bi[i] < 0:
+            raise ValueError(f"pool {i} is held by another rank")
+        b, j = self.buckets[bi[i]], int(loc[i])
+        z, g = float(b.logrw[2, j]), float(b.gamma[j])
+        return _bin_fills(self._bins().records(i), int(z), g, t)
+
     def update_pools(self, pool_ids, reserves=None, fees=None, prices=None, ladders=None, amp=None, rates=None,
-                     curve_gamma=None):
-        """Set new reserves, fees, prices, ladders, amplifications and / or rates of some pools in place: the store then
+                     curve_gamma=None, bins=None):
+        """Set new reserves, fees, prices, ladders, bins, A and / or rates of some pools in place: the store then
         equals, bit for bit, a PoolStore built from a HostPools of the updated literals, without re-uploading the pools or
         rebuilding the blocked layout (which depends on the token ids only).  pool_ids: global pool indices (the order of
         the problem's local_indices); reserves[k]: the new reserve vector of pool pool_ids[k], with the pool's arity (an
@@ -1844,20 +1912,28 @@ class PoolStore:
         cfmm_ladder_splice rewrites the bucket's records into a second device buffer, which the bucket then uses: a
         ladders= update moves the bucket's records pointer, so a CUDA graph captured over this store must be captured
         again.  The device keeps two record buffers of the concentrated bucket from the first ladders= update on.
+        bins[k] = (prices, x, y) (price-bin pools only; with fees= for the same pools if wanted): the pool's whole new
+        state, the triple of HostPools.from_lists (instances.lb_bins or instances.order_book of its state after a swap, a
+        deposit or withdrawal, a changed book or a filled order); K may change (1 .. BINS_K_MAX), its tokens and which one
+        is token 0 may not.  Its records are made by bin_records, as from_lists does, and cfmm_bins_splice rewrites the
+        bucket's records like cfmm_ladder_splice: a bins= update also moves the bucket's records pointer, so a CUDA graph
+        captured over this store must be captured again.  The replaced pools' multipliers (theta_bar) restart at 0, a
+        fresh pool's.  A bins pool takes no reserves= (its reserves are derived from its bins).  store.bin_fills(i, t)
+        splits a trade over the pool's current bins.
 
         All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.from_lists and
         validate) raise ValueError before anything is written on the device or in the store's host state, and so does an
         entry the device check of the blocked bucket rejects.  Pools held by other ranks of a sharded store are skipped:
         give every rank the same full update.  The caller's HostPools is not modified: the store reads no host reserve or
         fee after construction, and keeps its own copies of the rates, amplifications (copied whole at the first amp= /
-        rates= update) and ladder records (a LadderSlab: appends, not copies of every record).  Synchronous.  Returns the
-        number of blocked tiles whose fee record was rebuilt.
+        rates= update), ladder and bin records (a LadderSlab each: appends, not copies of every record).  Synchronous.
+        Returns the number of blocked tiles whose fee record was rebuilt.
 
         A new block of the same market is then re-solved warm from the previous prices:
             store.update_pools(ids, reserves=new_R, fees=new_gamma)
             res = solve_pools(hp, utility, store=store, nu0=res.nu)"""
         u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees, prices,
-                              ladders, amp, rates, curve_gamma)
+                              ladders, amp, rates, curve_gamma, bins)
         bi, loc = self._pool_map()
         owner = bi[u.ids]
         plan = []
@@ -1865,7 +1941,7 @@ class PoolStore:
             e = np.nonzero(owner == k)[0]
             if len(e) == 0:
                 continue
-            if u.ladders is not None:                # concentrated pools only (checked): the splice takes them in order
+            if u.ladders is not None or u.bins is not None:   # concentrated / bins pools only (checked): in bucket order
                 e = e[np.argsort(loc[u.ids[e]], kind="stable")]
             rs = u.ptr[e][None, :] + np.arange(b.arity)[:, None]          # (arity, n) indices into the update's slots
             ids = u.ids[e]
@@ -1880,6 +1956,10 @@ class PoolStore:
                 rec, cnt, s, c, x, y = new_ladders([u.ladders[j] for j in e.tolist()])
                 n_total = b.n_rec + int(cnt.sum()) - int((self._ladders().T[ids] + 1).sum())
                 lad = (rec, cnt, np.stack([s, c, x, y], 1), n_total)
+            if u.bins is not None:                   # new records and (z, p_ref, sum x, sum y), as from_lists makes them
+                rec, cnt, state = _pack_bins([u.bins[j] for j in e.tolist()])
+                n_total = b.n_rec + int(cnt.sum()) - int((self._bins().T[ids] + 1).sum())
+                lad = (rec, cnt, state, n_total)
             if u.amp is not None or u.rates is not None or u.curve_gamma is not None:
                 # StableSwap or cryptoswap pools only (checked): D of the reserves after the call
                 A = u.amp[e] if u.amp is not None else self._amp_host[ids]
@@ -1904,7 +1984,7 @@ class PoolStore:
             if getattr(b, "blocked", False):
                 continue
             if lad is not None:
-                b.splice_ladders(self.lib, l, lad[0], lad[1], lad[2], lad[3], self._stream())
+                b.splice_records(self.lib, l, lad[0], lad[1], lad[2], lad[3], self._stream())
             W = self._weights_host[u.slots[rs]] if (R is not None and b.logrw is not None and AD is None) else None
             crypto = b.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3)
             amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) or crypto else None
@@ -1913,7 +1993,7 @@ class PoolStore:
         # the store's host state, once the device holds the update
         for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:
             if lad is not None:
-                self._ladders().replace(ids, lad[0], lad[1])
+                (self._bins() if b.kind == _lib.KIND_BINS else self._ladders()).replace(ids, lad[0], lad[1])
             if AD is not None:
                 if not self._own_stable:
                     self._weights_host, self._amp_host = self._weights_host.copy(), self._amp_host.copy()

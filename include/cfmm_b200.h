@@ -270,6 +270,20 @@ int cfmm_ladder_splice(const cfmm_bucket* b, int64_t n_chg, const int64_t* pos, 
                        int64_t n_records, const double* state, double* out_records, int64_t out_capacity,
                        int64_t* status_host, void* work, int64_t work_bytes, void* stream);
 
+/*
+ * New bins for n_chg pools of a CFMM_KIND_BINS bucket (a swap that empties the active bin, a deposit or withdrawal, a
+ * changed book level, a filled limit order; K may change), spliced into a second record buffer.  The arguments and the
+ * all-or-nothing contract of cfmm_ladder_splice, with: n_rec [n_chg] = the new record counts nb (2 .. 2^20 + 2);
+ * records = their new records in the AoS layout of CFMM_KIND_BINS; state [n_chg][4] = their new (z, p_ref, sum x,
+ * sum y).  logrw rows 0-1 (first record, nb) of every pool and rows 2-3 (z, p_ref) and the reserves (sum x, sum y) of the
+ * changed pools are written in place; theta_bar is not touched (a caller that wants a replaced pool to start from a
+ * fresh pool's multiplier zeroes its row-0 entry).  work: cfmm_ladder_splice_work_bytes(b->n_pools, n_chg) bytes (the
+ * scans are the same).  CFMM_E_KIND unless kind BINS, arity 2.  SYNCHRONOUS on `stream`.
+ */
+int cfmm_bins_splice(const cfmm_bucket* b, int64_t n_chg, const int64_t* pos, const int64_t* n_rec, const double* records,
+                     int64_t n_records, const double* state, double* out_records, int64_t out_capacity,
+                     int64_t* status_host, void* work, int64_t work_bytes, void* stream);
+
 /* Same contract as cfmm_arb_eval for a blocked constant-product bucket: psi/arb ACCUMULATE (one red.add per row
  * of <= 32 entries, ~0.35 per pool, instead of 2 per pool).  Per-pool outputs (delta/lambda [2][n_tiles*P], hcoef
  * [n_tiles*P]) are in BLOCKED order.  If zero_next != NULL the launch also clears zero_next[0..n_zero): callers that
