@@ -110,8 +110,10 @@ def solve(local_indices, reserves, fees, kinds, weights=None, utility=None, n_to
     weights[i] = (price, bounds, liquidity), a whole Uniswap-v3 tick ladder as one pool, with reserves[i] = None (see
     HostPools.from_lists and instances.v3_ladder).  And 'cryptoswap': weights[i] = (A, gamma, p_0, p_1), a two-coin Curve v2
     (twocrypto-ng) pool with the whitepaper A, the curve's gamma and the price scales (see HostPools.from_lists and
-    instances.twocrypto_pool).  Problems with StableSwap, concentrated or cryptoswap pools run solver.py or the per-thread
-    solver, never the native blocked and persistent solvers."""
+    instances.twocrypto_pool).  And 'eclp': reserves[i] = (x, y), weights[i] = (alpha, beta, c, s, lam), a Gyroscope
+    elliptic concentrated-liquidity pool (see HostPools.from_lists and instances.eclp_pool).  Problems with StableSwap,
+    concentrated, cryptoswap or E-CLP pools run solver.py, the native host loop or the per-thread solver, never the native
+    blocked and persistent solvers."""
     if utility is None:
         raise ValueError("utility is required: Arbitrage(c) | Liquidate(target, assets) | Swap(i, o, t)")
     if n_tokens is None:

@@ -14,8 +14,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .pools import HostPools, KIND_BINS_HOST, KIND_CONCENTRATED_HOST, KIND_CRYPTOSWAP_HOST, KIND_GEOMEAN_HOST, \
-    KIND_STABLESWAP_HOST
+from .pools import HostPools, KIND_BINS_HOST, KIND_CONCENTRATED_HOST, KIND_CRYPTOSWAP_HOST, KIND_ECLP_HOST, \
+    KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
 from .solver import default_nu0
 
 NTOK_MAX = 64      # cfmm_small::NTOK_MAX
@@ -82,6 +82,18 @@ class CsrStore:
             self.logrw[first + 1] = torch.as_tensor((bp[bn + 1] - bp[bn]).astype(np.float64), device=dev)
             self.records = torch.as_tensor(np.concatenate([np.asarray(hp.lad_rec, np.float64).reshape(-1),
                                                            np.asarray(hp.bin_rec, np.float64).reshape(-1)]), device=dev)
+        ec = np.nonzero(np.asarray(hp.kind) == KIND_ECLP_HOST)[0]
+        self.has_eclp = bool(len(ec))                # -> cfmm_batch_solve_eclp (an eighth instance)
+        if len(ec):                                  # E-CLP pools: one record {c, s, lam, alpha, beta, r, p, 0} each after
+            lad = np.asarray(hp.lad_rec, np.float64).reshape(-1)      # the ladders' and bins' records, its index (units
+            bns = np.asarray(hp.bin_rec, np.float64).reshape(-1)      # of 4 f64) in the pool's first logrw slot
+            E = np.asarray(hp.eclp, np.float64)[ec]
+            rec = np.zeros((len(ec), 8))
+            rec[:, 0:3], rec[:, 3:5], rec[:, 5:7] = E[:, 2:5], E[:, 0:2], E[:, 5:7]
+            first = torch.as_tensor(np.asarray(hp.pool_ptr)[ec], device=dev)
+            at = (len(lad) + len(bns)) // 4 + 2 * np.arange(len(ec))
+            self.logrw[first] = torch.as_tensor(at.astype(np.float64), device=dev)
+            self.records = torch.as_tensor(np.concatenate([lad, bns, rec.reshape(-1)]), device=dev)
         cs = np.nonzero(np.asarray(hp.kind) == KIND_CRYPTOSWAP_HOST)[0]
         ptr = np.asarray(hp.pool_ptr, np.int64)
         c3 = cs[ptr[cs + 1] - ptr[cs] == 3]
@@ -153,6 +165,10 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if store.has_eclp:
+        _lib.check(store.lib.cfmm_batch_solve_eclp(C.byref(store.c_pools), store.records.data_ptr(), C.byref(batch),
+                                                   C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve_eclp")
+        return psi, stats, delta, lam
     if store.has_bins:
         _lib.check(store.lib.cfmm_batch_solve_bins(C.byref(store.c_pools), store.records.data_ptr(), C.byref(batch),
                                                    C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve_bins")
@@ -263,7 +279,8 @@ def pack_problems(problems: Sequence):
                        np.concatenate([np.asarray(hp.lad_sc, np.float64).reshape(-1, 2) for hp, _ in problems]),
                        cat("cgam", np.float64), np.concatenate(bptr),
                        np.concatenate([np.asarray(hp.bin_rec, np.float64).reshape(-1, 4) for hp, _ in problems]),
-                       np.concatenate([np.asarray(hp.bin_zp, np.float64).reshape(-1, 2) for hp, _ in problems]))
+                       np.concatenate([np.asarray(hp.bin_zp, np.float64).reshape(-1, 2) for hp, _ in problems]),
+                       np.concatenate([np.asarray(hp.eclp, np.float64).reshape(-1, 7) for hp, _ in problems]))
     return merged, ranges, c, a, fl, nu, nnz_max
 
 

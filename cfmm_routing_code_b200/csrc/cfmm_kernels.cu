@@ -9,7 +9,7 @@
 #include <math.h>
 
 #include "cfmm_dev.cuh"
-#include "cfmm_small.cuh"     // bounded_pair(), ladder_pair(), bins_pair(), ...: the per-pool math, shared with the per-thread solver
+#include "cfmm_small.cuh"     // bounded_pair(), eclp_pair(), ladder_pair(), bins_pair(), ...: the per-pool math, shared with the per-thread solver
 
 namespace cfmm {
 std::atomic<long long> g_launches{0};
@@ -143,6 +143,17 @@ k_eval_pair(long long m, long long ld, int n_tokens, const double* __restrict__ 
             // `thbar` carries the per-slot auxiliary array of the bucket: here the virtual-reserve offsets
             double D[2], L[2];
             cfmm_small::bounded_pair(R0, R1, thbar[i], thbar[ld + i], g, n0, n1, D, L, h);
+            y0 = L[0] - D[0];
+            y1 = L[1] - D[1];
+            if (TRADES) {
+                delta[i] = D[0]; delta[ld + i] = D[1];
+                lambda[i] = L[0]; lambda[ld + i] = L[1];
+            }
+        } else if (KIND == CFMM_KIND_ECLP) {
+            // `thbar` carries the bucket's weights [7][ld] = (alpha, beta, c, s, lam, r, p)
+            double D[2], L[2];
+            cfmm_small::eclp_pair(R0, R1, thbar[i], thbar[ld + i], thbar[2 * ld + i], thbar[3 * ld + i],
+                                  thbar[4 * ld + i], thbar[5 * ld + i], thbar[6 * ld + i], g, n0, n1, D, L, h);
             y0 = L[0] - D[0];
             y1 = L[1] - D[1];
             if (TRADES) {
@@ -920,10 +931,12 @@ int launch_pair(const cfmm_bucket* b, int n_tokens, const double* nu, double eps
     double* delta = out ? out->delta : nullptr;
     double* lambda = out ? out->lambda : nullptr;
     double* hcoef = out ? out->hcoef : nullptr;
-    // per-slot auxiliary array: fill multipliers of constant-sum orders | virtual-reserve offsets of bounded products
-    const double* aux = KIND == CFMM_KIND_BOUNDED_PRODUCT ? b->weights : b->theta_bar;
-    if (KIND != CFMM_KIND_BOUNDED_PRODUCT && (g_scatter_mode == 0 || g_scatter_mode == 3) && tma_ok(b)) {
-        auto kern = k_eval_pair_tma<KIND == CFMM_KIND_BOUNDED_PRODUCT ? CFMM_KIND_PRODUCT : KIND, TRADES, HESS>;
+    // per-slot auxiliary array: fill multipliers of constant-sum orders | virtual-reserve offsets of bounded products |
+    // the parameters and state of E-CLPs.  Neither of the last two has a TMA-staged kernel: the LDG path only.
+    constexpr bool kWeights = KIND == CFMM_KIND_BOUNDED_PRODUCT || KIND == CFMM_KIND_ECLP;
+    const double* aux = kWeights ? b->weights : b->theta_bar;
+    if (!kWeights && (g_scatter_mode == 0 || g_scatter_mode == 3) && tma_ok(b)) {
+        auto kern = k_eval_pair_tma<kWeights ? CFMM_KIND_PRODUCT : KIND, TRADES, HESS>;
         const size_t sm = (size_t)kStages * kStageBytes;
         static bool attr_set = false;      // per instantiation
         if (!attr_set) {
@@ -1205,6 +1218,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 2) return CFMM_E_KIND;
             if (b->n_pools > 0 && (!b->weights || !b->logrw || !b->theta_bar)) return CFMM_E_NULL;   // records; tbar
             break;
+        case CFMM_KIND_ECLP:
+            if (b->arity != 2) return CFMM_E_KIND;
+            if (b->n_pools > 0 && !b->weights) return CFMM_E_NULL;       // (alpha, beta, c, s, lam, r, p)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -1240,6 +1257,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_CRYPTOSWAP>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_BINS:
             return dispatch_pair<CFMM_KIND_BINS>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_ECLP:
+            return dispatch_pair<CFMM_KIND_ECLP>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_CRYPTOSWAP_3:
             return dispatch_crypto3(b, n_tokens, nu, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP_N:

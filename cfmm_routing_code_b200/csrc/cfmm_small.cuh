@@ -104,6 +104,76 @@ CFMM_HD inline void bounded_pair(double R0, double R1, double o0, double o1, dou
     }
 }
 
+// Elliptic concentrated-liquidity pool (Gyroscope E-CLP; not a reference atom).  Price range [alpha, beta] (token 1 per
+// token 0), rotation (c, s) = (cos phi, sin phi), stretch lam >= 1; A = [[c/lam, -s/lam], [s, c]], M = (A'A)^-1 with
+// M00 = s^2 + lam^2 c^2, M01 = -cs (lam^2 - 1), det M = lam^2.  The pool keeps ||A (t - r chi)|| <= r, t >= 0; its
+// boundary is t(p) = r (chi - f(p)), p in [alpha, beta], f(p) = M (p, 1)' / h(p), h(p)^2 = (p, 1) M (p, 1)', and the
+// marginal price at t(p) is p.  The pool's state is (r, p): the invariant and the price of its balances.
+// Every flow is a difference t(q) - t(p) written as (p - q) times a positive quotient, never a difference of points:
+//   f_x(p1) - f_x(p2) = (p1 - p2) B(p1, p2),  B = (Tx + D) / (h1 h2 (h1 + h2)),  D = lam^2,
+//   f_y(p2) - f_y(p1) = (p1 - p2) C(p1, p2),  C = (Ty + D p1 p2) / (h1 h2 (h1 p2 + h2 p1)),
+//   gx(p) = M00 p + M01 = lam^2 c (c p - s) + s (s p + c),  gy(p) = M01 p + M11 = c (s p + c) - lam^2 s (c p - s)
+//   (c p - s by one fma: no lam^2 cancellation near the peg s / c),  h^2 = (gx^2 + D) / M00,
+//   Tx = M00 h1 h2 - gx1 gx2 = D (gx1^2 + gx2^2 + D) / (M00 h1 h2 + gx1 gx2)  (the latter if gx1 gx2 > 0),
+//   Ty = M11 h1 h2 - gy1 gy2 = D (gy1^2 p2^2 + gy2^2 p1^2 + D p1^2 p2^2) / (M11 h1 h2 + gy1 gy2)  (if gy1 gy2 > 0).
+// C is B of the mirrored pool (tokens swapped, p -> 1/p, (c, s) -> (s, c)) at (1/p1, 1/p2), over p1 p2, written in p:
+// rounding 1/p would cost up to p / |p - s/c| ulp of the flow near the peg when lam is large.
+CFMM_HD inline double eclp_h(double c, double s, double D, double p) {
+    const double g = D * c * fma(c, p, -s) + s * fma(s, p, c);
+    return sqrt(fma(g, g, D) / fma(D * c, c, s * s));
+}
+
+CFMM_HD inline void eclp_BC(double c, double s, double D, double p1, double p2, double& B, double& C) {
+    const double M00 = fma(D * c, c, s * s), M11 = fma(D * s, s, c * c);
+    const double e1 = fma(c, p1, -s), e2 = fma(c, p2, -s), o1 = fma(s, p1, c), o2 = fma(s, p2, c);
+    const double gx1 = D * c * e1 + s * o1, gx2 = D * c * e2 + s * o2;
+    const double gy1 = c * o1 - D * s * e1, gy2 = c * o2 - D * s * e2;
+    const double h1 = sqrt(fma(gx1, gx1, D) / M00), h2 = sqrt(fma(gx2, gx2, D) / M00);
+    const double hh = h1 * h2;
+    const double xx = gx1 * gx2, yy = gy1 * gy2, q12 = p1 * p2;
+    const double Tx = xx > 0.0 ? D * (fma(gx1, gx1, fma(gx2, gx2, D)) / fma(M00, hh, xx)) : fma(M00, hh, -xx);
+    const double Ty = yy > 0.0 ? D * (fma(gy1 * p2, gy1 * p2, fma(gy2 * p1, gy2 * p1, D * q12 * q12)) / fma(M11, hh, yy))
+                               : fma(M11, hh, -yy);
+    B = (Tx + D) / (hh * (h1 + h2));
+    C = fma(D, q12, Ty) / (hh * fma(h1, p2, h2 * p1));
+}
+
+// The optimal trade at prices (n0, n1) of the pool (x, y) = the reserves at its state (r, p), fee gam.  Tender 0 iff
+// p* = n0 / (gam n1) < p: the price falls to q = max(p*, alpha), D_0 = r (p - q) B(p, q) / gam, L_1 = r (p - q) C(p, q)
+// (= y at q = alpha).  Tender 1 iff p* = gam n0 / n1 > p: the price rises to q = min(p*, beta), L_0 = r (q - p) B(p, q)
+// (= x at q = beta), D_1 = r (q - p) C(p, q) / gam.  hc = r lam^2 n1 p*^2 / h(p*)^3, over gam when tendering 1, 0 at a
+// cap or with no trade.
+CFMM_HD inline void eclp_pair(double x, double y, double alpha, double beta, double c, double s, double lam, double r,
+                              double p, double gam, double n0, double n1, double* Dl, double* Ll, double& hc) {
+    Dl[0] = Dl[1] = Ll[0] = Ll[1] = 0.0;
+    hc = 0.0;
+    const double D = lam * lam;
+    const double lo = n0 / (gam * n1), hi = gam * n0 / n1;
+    const bool t0 = lo < p, t1 = hi > p;
+    if (!t0 && !t1) return;
+    const double ps = t0 ? lo : hi;
+    const bool cap = t0 ? ps <= alpha : ps >= beta;
+    const double q = cap ? (t0 ? alpha : beta) : ps;
+    const double dq = t0 ? p - q : q - p;                                   // >= 0
+    double B, C;
+    eclp_BC(c, s, D, p, q, B, C);
+    // token 0 and token 1 moved along the arc; at a cap the side paid out is the whole reserve, exactly
+    const double fx = t1 && cap ? x : r * dq * B;
+    const double fy = t0 && cap ? y : r * dq * C;
+    if (t0) {
+        Dl[0] = fx / gam;
+        Ll[1] = fy;
+    } else {
+        Ll[0] = fx;
+        Dl[1] = fy / gam;
+    }
+    if (!cap) {
+        const double h = eclp_h(c, s, D, ps);
+        hc = r * D * n1 * ps * ps / (h * h * h);
+        if (t1) hc /= gam;
+    }
+}
+
 // Concentrated-liquidity pool (a whole Uniswap-v3 tick ladder): sqrt-price bounds b_0 < ... < b_T, liquidity L_k on
 // [b_k, b_{k+1}), current sqrt price s in [b_0, b_T] inside interval c (b_c <= s, c <= T - 1).  One record per bound,
 // rec[4k .. 4k+3] = {b_k, L_k, Y_k, X_k}: Y_k = sum_{j<k} L_j (b_{j+1} - b_j) (token 1 below b_k), X_k =
@@ -979,8 +1049,11 @@ CFMM_UNROLL
 // BINS (with all five): also price-bin pools (kind 10) through bins_pair, (z, p_ref) in the pool's two w slots, (first
 // record, nb) in its two logrw slots, the records in `rec` (shared with the concentrated pools') and the multiplier tbar in
 // its first theta_bar slot; cfmm_batch_solve_bins runs this seventh instance.  The others give such problems status 3.
+// ECLP (with all six): also E-CLP pools (kind 11) through eclp_pair, their record {c, s, lam, alpha, beta, r, p, 0} (two
+// record slots) in `rec` after the ladders' and bins', its record index in the pool's first logrw slot;
+// cfmm_batch_solve_eclp runs this eighth instance.  The others give such problems status 3.
 template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
-          bool CRYPTO3 = false, bool BINS = false>
+          bool CRYPTO3 = false, bool BINS = false, bool ECLP = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane,
                                const double* rec = nullptr) {
@@ -1058,6 +1131,16 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
                         }
                     }
                 }
+            }
+        } else if (ECLP && P.kind[i] == 11) {                         // {c, s, lam, alpha, beta, r, p, 0} in rec
+            double hc = 0.0;
+            const double* e = rec + 4 * (int64_t)P.logrw[off];
+            eclp_pair(P.R[off], P.R[off + 1], e[3], e[4], e[0], e[1], e[2], e[5], e[6], gam, nu[P.tok[off]],
+                      nu[P.tok[off + 1]], D, L, hc);
+            if (Hs && hc != 0.0) {
+                const int t0 = P.tok[off], t1 = P.tok[off + 1];
+                (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
+                (*Hs)[t0 * n + t1] -= hc; (*Hs)[t1 * n + t0] -= hc;
             }
         } else if (P.kind[i] == 3 || (STABLE && P.kind[i] == 4)) {
             double hc = 0.0;
@@ -1259,7 +1342,7 @@ CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
 // rec: the concentrated and price-bin pools' records (LADDER and BINS instances only).
 template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
-          bool CRYPTO3 = false, bool BINS = false>
+          bool CRYPTO3 = false, bool BINS = false, bool ECLP = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0, const double* rec = nullptr) {
     const int n = Q.n;
@@ -1280,9 +1363,10 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1 || (BINS && P.kind[i] == 10);
         bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6) && !(CRYPTO && P.kind[i] == 8) &&
-               !(CRYPTO3 && P.kind[i] == 9) && !(BINS && P.kind[i] == 10)) || k < 2 ||
+               !(CRYPTO3 && P.kind[i] == 9) && !(BINS && P.kind[i] == 10) && !(ECLP && P.kind[i] == 11)) || k < 2 ||
               k > KMAX || ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
-                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8) || (BINS && P.kind[i] == 10)) && k != 2) ||
+                (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8) || (BINS && P.kind[i] == 10) ||
+                (ECLP && P.kind[i] == 11)) && k != 2) ||
               (CRYPTO3 && P.kind[i] == 9 && k != 3);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
@@ -1310,7 +1394,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -1356,7 +1440,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -1381,8 +1465,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -1415,8 +1499,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

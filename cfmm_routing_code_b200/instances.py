@@ -539,6 +539,59 @@ def synth_tricrypto_market(m, n_tokens, seed, frac_tri=0.3, far=0.5, mispricing=
     return hp, p
 
 
+def eclp_pool(balances, decimals, params, rates=(1, 1)):
+    """A Balancer GyroECLP pool's state as ("eclp" reserves, weights): balances = the two raw token balances, decimals
+    their token decimals, params = the pool's 18-decimal (alpha, beta, c, s, lambda) integers, rates = its rate providers'
+    rates (1 without providers; 18-decimal integers are divided by 1e18 when given as int >= 1e9).  The pool prices its
+    balances scaled by the rates, so reserves = balance / 10^decimals * rate (units of the rate-scaled tokens) and the
+    price range stays the pool's.  Agreement with the contract's fixed-point calculateInvariantWithError is not verified
+    (INTEGRATION.md)."""
+    from decimal import Decimal
+    rt = [Decimal(int(r)) / Decimal(10) ** 18 if isinstance(r, int) and r >= 10 ** 9 else Decimal(str(r)) for r in rates]
+    res = [float(Decimal(int(b)) / Decimal(10) ** int(d) * r) for b, d, r in zip(balances, decimals, rt)]
+    w = tuple(float(Decimal(int(v)) / Decimal(10) ** 18) for v in params)
+    return res, w
+
+
+def synth_eclp_market(m, n_tokens, seed, frac_eclp=0.3, lam=(1.0, 1e4), mispricing=0.02):
+    """A market of E-CLP pools beside every other kind: a frac_eclp share of m pools are E-CLPs on random token pairs,
+    their peg at the market price (off by `mispricing`), ranges 0.5 % .. 50 % either side, stretch lam log-uniform in
+    `lam`, fees 0.01 .. 0.3 %, balances at a price inside the range; the rest is synth_tricrypto_market's mix (every
+    other kind but bins).  n_tokens >= 3.  Returns (HostPools, prices)."""
+    from .pools import HostPools, KIND_ECLP_HOST, _eclp_xy, eclp_state
+    rng = np.random.default_rng(seed + 7919)
+    n_e = int(round(frac_eclp * m))
+    base, p = synth_tricrypto_market(m - n_e, n_tokens, seed, mispricing=mispricing)
+    a = rng.integers(0, n_tokens, n_e)
+    b = (a + rng.integers(1, n_tokens, n_e)) % n_tokens
+    mid = p[a] / p[b] * np.exp(mispricing * rng.standard_normal(n_e))       # token b per token a
+    phi = np.arctan(mid)
+    c, s = np.cos(phi), np.sin(phi)
+    h = np.hypot(c, s)
+    c, s = c / h, s / h
+    alpha = mid * (1 - np.exp(rng.uniform(np.log(5e-3), np.log(0.5), n_e)))
+    beta = mid * (1 + np.exp(rng.uniform(np.log(5e-3), np.log(0.5), n_e)))
+    L = np.exp(rng.uniform(np.log(lam[0]), np.log(lam[1]), n_e))
+    P = np.stack([alpha, beta, c, s, L], axis=1)
+    pc = mid * np.exp(0.5 * mispricing * rng.standard_normal(n_e)).clip(alpha / mid * 1.0001, beta / mid * 0.9999)
+    X, Y = _eclp_xy(alpha, beta, c, s, L * L, pc)
+    r = np.exp(9.0 + 1.5 * rng.standard_normal(n_e)) / p[b] / np.maximum(Y + X * mid, 1e-300)
+    R = np.stack([r * X, r * Y], axis=1)
+    st = eclp_state(R, P)
+    gam = np.array([0.9999, 0.9995, 0.999, 0.997])[rng.integers(0, 4, n_e)]
+    z2 = lambda k: np.zeros((n_e, k))
+    hp = HostPools(n_tokens, np.concatenate([base.pool_ptr, base.pool_ptr[-1] + 2 * np.arange(1, n_e + 1)]).astype(np.int64),
+                   np.concatenate([base.tok_idx, np.stack([a, b], 1).ravel()]).astype(np.int32),
+                   np.concatenate([base.reserves, R.ravel()]), np.concatenate([base.weights, np.zeros(2 * n_e)]),
+                   np.concatenate([base.gamma, gam]),
+                   np.concatenate([base.kind, np.full(n_e, KIND_ECLP_HOST, np.uint8)]).astype(np.uint8),
+                   np.concatenate([base.amp, np.zeros(n_e)]), np.concatenate([base.inv, np.zeros(n_e)]),
+                   np.concatenate([base.lad_ptr, np.full(n_e, base.lad_ptr[-1], np.int64)]), base.lad_rec,
+                   np.concatenate([base.lad_sc, z2(2)]), np.concatenate([np.asarray(base.cgam, float), np.zeros(n_e)]),
+                   eclp=np.concatenate([np.zeros((base.m, 7)), np.concatenate([P, st], axis=1)]))
+    return hp, p
+
+
 LB_ID_OFFSET = 1 << 23      # Liquidity Book's bin id of price 1 (raw units)
 
 

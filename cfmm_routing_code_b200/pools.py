@@ -30,6 +30,98 @@ CRYPTO_A_RANGE = (1e-6, 1e4)       # accepted whitepaper A of cryptoswap pools (
 CRYPTO_GAMMA_RANGE = (1e-6, 0.1)   # accepted curve gamma of cryptoswap pools (tests/test_cryptoswap.py checks the corners)
 LADDER_T_MAX = 1 << 20  # most intervals of one concentrated pool (cfmm_small::LADDER_T_MAX)
 BINS_K_MAX = 1 << 20    # most bins of one price-bin pool (cfmm_small::BINS_K_MAX)
+KIND_ECLP_HOST = 11     # elliptic concentrated liquidity (Gyroscope E-CLP); (alpha, beta, c, s, lam, r, p) in HostPools.eclp
+ECLP_LAM_MAX = 1e8      # largest stretch lam of an E-CLP
+
+
+def _two_prod(a, b):
+    """a * b = p + e exactly (Dekker's split; numpy has no fma)"""
+    p = a * b
+    sp = 134217729.0                                    # 2^27 + 1
+    ta, tb = sp * a, sp * b
+    ah = ta - (ta - a); al = a - ah
+    bh = tb - (tb - b); bl = b - bh
+    return p, ((ah * bh - p) + ah * bl + al * bh) + al * bl
+
+
+def _eclp_BC(c, s, D, p1, p2):
+    """the quotients B = (f_x(p1) - f_x(p2)) / (p1 - p2) and C = (f_y(p2) - f_y(p1)) / (p1 - p2), cancellation free
+    (cfmm_small::eclp_BC; c p - s from an exact product, as the fma there)"""
+    M00, M11 = D * c * c + s * s, D * s * s + c * c
+
+    def cps(p):
+        hi, lo = _two_prod(c, p)
+        return (hi - s) + lo
+    e1, e2, o1, o2 = cps(p1), cps(p2), s * p1 + c, s * p2 + c
+    gx1, gx2 = D * c * e1 + s * o1, D * c * e2 + s * o2
+    gy1, gy2 = c * o1 - D * s * e1, c * o2 - D * s * e2
+    h1, h2 = np.sqrt((gx1 * gx1 + D) / M00), np.sqrt((gx2 * gx2 + D) / M00)
+    hh, xx, yy, q12 = h1 * h2, gx1 * gx2, gy1 * gy2, p1 * p2
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        Tx = np.where(xx > 0, D * ((gx1 * gx1 + (gx2 * gx2 + D)) / (M00 * hh + xx)), M00 * hh - xx)
+        Ty = np.where(yy > 0, D * (((gy1 * p2) ** 2 + ((gy2 * p1) ** 2 + D * q12 * q12)) / (M11 * hh + yy)),
+                      M11 * hh - yy)
+    return (Tx + D) / (hh * (h1 + h2)), (D * q12 + Ty) / (hh * (h1 * p2 + h2 * p1))
+
+
+def _eclp_xy(alpha, beta, c, s, D, p):
+    """balances per unit r at price p: x = (beta - p) B(beta, p), y = (p - alpha) C(alpha, p)"""
+    return (beta - p) * _eclp_BC(c, s, D, beta, p)[0], (p - alpha) * _eclp_BC(c, s, D, alpha, p)[1]
+
+
+def eclp_state(reserves, params) -> np.ndarray:
+    """(r, p) of E-CLP pools: the invariant r and the price p (token 1 per token 0) of the balances reserves [m, 2] =
+    (x, y), params [m, 5] = (alpha, beta, c, s, lam).  p is the root of x Y(p) = y X(p) on [alpha, beta] (X, Y the balances
+    per unit r, _eclp_xy), found by bisection to adjacent doubles (p = beta iff x = 0, p = alpha iff y = 0); r comes from
+    the coordinate that is the larger share of its range.  Gyroscope's quadratic for r is not used: its leading
+    coefficient cancels in fp64 when the peg s / c lies outside the range.  Returns [m, 2] = (r, p)."""
+    R = np.asarray(reserves, np.float64).reshape(-1, 2)
+    P = np.asarray(params, np.float64).reshape(-1, 5)
+    x, y = R[:, 0], R[:, 1]
+    a, b, c, s, lam = (P[:, k] for k in range(5))
+    D = lam * lam
+    lo, hi = a.copy(), b.copy()
+    live = (x > 0) & (y > 0)
+    for _ in range(2100):                                # enough for any pair of doubles
+        if not live.any():
+            break
+        mid = lo + 0.5 * (hi - lo)
+        X, Y = _eclp_xy(a, b, c, s, D, mid)
+        up = x * Y < y * X                              # the root lies above mid
+        lo = np.where(live & up, mid, lo)
+        hi = np.where(live & ~up, mid, hi)
+        nxt = lo + 0.5 * (hi - lo)
+        live &= (nxt != lo) & (nxt != hi)               # lo, hi adjacent: done
+    Xl, Yl = _eclp_xy(a, b, c, s, D, lo)
+    Xh, Yh = _eclp_xy(a, b, c, s, D, hi)
+    p = np.where(np.abs(x * Yl - y * Xl) <= np.abs(x * Yh - y * Xh), lo, hi)
+    p = np.where(x == 0, b, np.where(y == 0, a, p))
+    X, Y = _eclp_xy(a, b, c, s, D, p)
+    X0, _ = _eclp_xy(a, b, c, s, D, a)
+    _, Y1 = _eclp_xy(a, b, c, s, D, b)
+    use_x = X * Y1 >= Y * X0
+    with np.errstate(divide="ignore", invalid="ignore"):
+        r = np.where(use_x, x / X, y / Y)
+    return np.stack([r, p], axis=1)
+
+
+def _check_eclp(params, reserves, where=""):
+    """The value rules of E-CLP pools: 0 < alpha < beta finite, c, s >= 0 with |c^2 + s^2 - 1| <= 1e-12,
+    1 <= lam <= ECLP_LAM_MAX, reserves finite, >= 0 and not both 0.  Returns params with (c, s) normalised by hypot."""
+    P = np.array(params, np.float64).reshape(-1, 5)
+    R = np.asarray(reserves, np.float64).reshape(-1, 2)
+    a, b, c, s, lam = (P[:, k] for k in range(5))
+    if not bool(np.all(np.isfinite(P)) and np.all((a > 0) & (a < b))):
+        raise ValueError(f"{where}eclp needs a finite price range 0 < alpha < beta")
+    if not bool(np.all((c >= 0) & (s >= 0) & (np.abs(c * c + s * s - 1.0) <= 1e-12))):
+        raise ValueError(f"{where}eclp needs c = cos(phi), s = sin(phi) >= 0 with |c^2 + s^2 - 1| <= 1e-12")
+    if not bool(np.all((lam >= 1) & (lam <= ECLP_LAM_MAX))):
+        raise ValueError(f"{where}eclp stretch lam must lie in [1, {ECLP_LAM_MAX:g}]")
+    if not bool(np.all(np.isfinite(R) & (R >= 0)) and np.all((R[:, 0] > 0) | (R[:, 1] > 0))):
+        raise ValueError(f"{where}eclp reserves must be finite, >= 0 and not both 0")
+    h = np.hypot(c, s)
+    P[:, 2], P[:, 3] = c / h, s / h
+    return P
 
 
 def ladder_records(bounds, liquidity) -> np.ndarray:
@@ -490,9 +582,14 @@ class HostPools:
     bin_ptr: Optional[np.ndarray] = None   # int64 [m+1]
     bin_rec: Optional[np.ndarray] = None   # f64 [n_records, 4]
     bin_zp: Optional[np.ndarray] = None    # f64 [m, 2]
+    # E-CLP pools (kind 11): eclp[i] = (alpha, beta, c, s, lam, r, p), the parameters with (c, s) normalised and the state
+    # of the reserves (eclp_state); 0 on other kinds.  Their weights are 0.  None: no E-CLP pools.
+    eclp: Optional[np.ndarray] = None      # f64 [m, 7]
 
     def __post_init__(self):
         m = len(self.gamma)
+        if self.eclp is None:
+            self.eclp = np.zeros((m, 7))
         if self.bin_ptr is None:
             self.bin_ptr = np.zeros(m + 1, np.int64)
         if self.bin_rec is None:
@@ -542,7 +639,11 @@ class HostPools:
         limit orders): weights[i] = (prices, x, y) with the K bins' prices in token 1 per token 0 (the caller's units),
         strictly increasing, and their holdings x of token 0 and y of token 1, finite, >= 0, not all 0, uncrossed (every
         bin with y > 0 prices at or below every bin with x > 0), 1 <= K <= BINS_K_MAX; reserves[i] must be None (they are
-        (sum x, sum y)).  instances.lb_bins and instances.order_book build the triple."""
+        (sum x, sum y)).  instances.lb_bins and instances.order_book build the triple.  And 'eclp' (an elliptic
+        concentrated-liquidity pool, Gyroscope E-CLP): reserves[i] = (x, y), finite, >= 0, not both 0; weights[i] =
+        (alpha, beta, c, s, lam) with the price range 0 < alpha < beta in token 1 per token 0, c = cos(phi), s = sin(phi)
+        >= 0 (|c^2 + s^2 - 1| <= 1e-12; normalised here), 1 <= lam <= ECLP_LAM_MAX; the state (r, p) comes from
+        eclp_state.  instances.eclp_pool converts a pool's on-chain state."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
@@ -551,8 +652,20 @@ class HostPools:
         cgam = np.zeros(m)
         lad = {}                                         # concentrated pool -> its records and price
         bins = {}                                        # bins pool -> bin_records
+        ecl = {}                                         # E-CLP pool -> its checked parameters
         for i, l in enumerate(local_indices):
             k = len(l)
+            if kinds[i] == "eclp":
+                if k != 2 or len(set(int(t) for t in l)) != 2:
+                    raise ValueError(f"pool {i}: eclp pools need 2 distinct tokens")
+                if reserves[i] is None or len(reserves[i]) != 2:
+                    raise ValueError(f"pool {i}: eclp needs reserves[i] = (x, y)")
+                if weights is None or weights[i] is None or len(weights[i]) != 5:
+                    raise ValueError(f"pool {i}: eclp needs weights[i] = (alpha, beta, c, s, lam)")
+                ecl[i] = _check_eclp(weights[i], reserves[i], f"pool {i}: ")[0]
+                ptr.append(ptr[-1] + 2); idx += [int(t) for t in l]; res += [float(x) for x in reserves[i]]
+                wts += [0.0, 0.0]; kd.append(KIND_ECLP_HOST)
+                continue
             if kinds[i] == "bins":
                 if k != 2 or len(set(int(t) for t in l)) != 2:
                     raise ValueError(f"pool {i}: bins pools need 2 distinct tokens")
@@ -636,10 +749,16 @@ class HostPools:
                 cnt[i] = len(b[0]); bin_zp[i] = (b[1], b[2])
             bin_ptr[1:] = np.cumsum(cnt)
             brec = np.concatenate([bins[i][0] for i in sorted(bins)])
+        eclp = np.zeros((m, 7))
+        if ecl:
+            ids = np.asarray(sorted(ecl), np.int64)
+            first = np.asarray(ptr, np.int64)[ids]
+            eclp[ids, :5] = np.stack([ecl[i] for i in ids.tolist()])
+            eclp[ids, 5:] = eclp_state(np.stack([res[first], res[first + 1]], axis=1), eclp[ids, :5])
         return HostPools(int(n_tokens), np.asarray(ptr, np.int64), np.asarray(idx, np.int32),
                          res, np.asarray(wts, np.float64),
                          np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp, None, lad_ptr,
-                         np.concatenate(recs) if recs else None, lad_sc, cgam, bin_ptr, brec, bin_zp)
+                         np.concatenate(recs) if recs else None, lad_sc, cgam, bin_ptr, brec, bin_zp, eclp)
 
     @staticmethod
     def from_pairs(n_tokens, idx, reserves, gamma) -> "HostPools":
@@ -664,16 +783,18 @@ class HostPools:
 
     def validate(self):
         slot_kind = np.repeat(np.asarray(self.kind), np.diff(self.pool_ptr)) if \
-            np.any((self.kind == KIND_BOUNDED_HOST) | (self.kind == KIND_CONCENTRATED_HOST) | (self.kind == KIND_BINS_HOST)) \
-            else None
+            np.any((self.kind == KIND_BOUNDED_HOST) | (self.kind == KIND_CONCENTRATED_HOST) | (self.kind == KIND_BINS_HOST)
+                   | (self.kind == KIND_ECLP_HOST)) else None
         virt = self.reserves if slot_kind is None else self.reserves + np.where(slot_kind == KIND_BOUNDED_HOST, self.weights, 0.0)
         lo_ok = np.all(self.reserves > 0) if slot_kind is None else np.all(self.reserves >= 0) and \
-            np.all((virt > 0) | (slot_kind == KIND_CONCENTRATED_HOST) | (slot_kind == KIND_BINS_HOST))
+            np.all((virt > 0) | (slot_kind == KIND_CONCENTRATED_HOST) | (slot_kind == KIND_BINS_HOST)
+                   | (slot_kind == KIND_ECLP_HOST))
         if not lo_ok or not np.all(np.isfinite(self.reserves)):
             raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves; "
-                             "concentrated, bins: >= 0)")
+                             "concentrated, bins, eclp: >= 0)")
         self._validate_ladders()
         self._validate_bins()
+        self._validate_eclp()
         if np.any(self.gamma <= 0) or np.any(self.gamma > 1):
             raise ValueError("fees (gamma) must lie in (0, 1]")
         if self.tok_idx.min(initial=0) < 0 or self.tok_idx.max(initial=0) >= self.n_tokens:
@@ -693,6 +814,27 @@ class HostPools:
             if not bool(np.all(np.isfinite(D) & (D > 0))):
                 raise ValueError("cryptoswap invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
 
+
+    def _validate_eclp(self):
+        """The rules of E-CLP pools on the CSR form: arity 2, the parameter rules of _check_eclp with (c, s) normalised,
+        and a state (r, p) with r finite and > 0, alpha <= p <= beta."""
+        ec = np.asarray(self.kind) == KIND_ECLP_HOST
+        E = np.asarray(self.eclp, np.float64)
+        if E.shape != (self.m, 7):
+            raise ValueError("eclp must be an [m, 7] array")
+        if not ec.any():
+            return
+        ids = np.nonzero(ec)[0]
+        if np.any(np.diff(self.pool_ptr)[ids] != 2):
+            raise ValueError("eclp pools must have 2 tokens")
+        first = np.asarray(self.pool_ptr, np.int64)[ids]
+        R = np.stack([self.reserves[first], self.reserves[first + 1]], axis=1)
+        _check_eclp(E[ids, :5], R)
+        if not bool(np.all(np.abs(np.hypot(E[ids, 2], E[ids, 3]) - 1.0) <= 4 * 2.0 ** -53)):
+            raise ValueError("eclp (c, s) must be normalised (c = cos(phi), s = sin(phi) by hypot)")
+        r, p = E[ids, 5], E[ids, 6]
+        if not bool(np.all(np.isfinite(r) & (r > 0) & (p >= E[ids, 0]) & (p <= E[ids, 1]))):
+            raise ValueError("eclp state (r, p): r finite and > 0, p in [alpha, beta] (eclp_state)")
 
     def _validate_bins(self):
         """The rules of price-bin pools on the CSR form: arity 2; 2 .. BINS_K_MAX + 2 records, none on other kinds; T
@@ -877,13 +1019,17 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
     if reserves is not None:
         R = _pool_rows(reserves, n, ar, "reserves")
         bounded = np.repeat(np.asarray(kind)[ids] == KIND_BOUNDED_HOST, ar)
-        if bounded.any():
+        ecl = np.asarray(kind)[ids] == KIND_ECLP_HOST
+        if bounded.any() or ecl.any():
+            es = np.repeat(ecl, ar)
             virt = R + np.where(bounded, weights[slots], 0.0)
-            ok = np.where(bounded, R >= 0, True) & (virt > 0)
+            ok = np.where(bounded | es, R >= 0, True) & ((virt > 0) | es)
+            ok = bool(np.all(ok)) and bool(np.all((R[first[:-1]] + R[np.minimum(first[:-1] + 1, len(R) - 1)] > 0)[ecl]))
         else:
             ok = R > 0
         if not (bool(np.all(ok)) and bool(np.all(np.isfinite(R)))):
-            raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves)")
+            raise ValueError("reserves must be positive and finite (bounded_product: >= 0 with positive virtual reserves; "
+                             "eclp: >= 0, not both 0)")
     g = None
     if fees is not None:
         g = np.ascontiguousarray(fees, np.float64).reshape(-1)
@@ -1042,6 +1188,11 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         if np.any(ar[bn] != 2):
             raise ValueError("bins pools must have 2 tokens")
         keys.append((_lib.KIND_BINS, 2, np.nonzero(bn)[0]))
+    ec = hp.kind == KIND_ECLP_HOST
+    if ec.any():
+        if np.any(ar[ec] != 2):
+            raise ValueError("eclp pools must have 2 tokens")
+        keys.append((_lib.KIND_ECLP, 2, np.nonzero(ec)[0]))
     cs = hp.kind == KIND_CRYPTOSWAP_HOST
     if cs.any():
         if np.any((ar[cs] != 2) & (ar[cs] != 3)):
@@ -1136,6 +1287,8 @@ class DeviceBucket:
             zp = np.asarray(hp.bin_zp, np.float64)[sel]
             P = np.stack([loc.astype(np.float64), cnt.astype(np.float64), zp[:, 0], zp[:, 1]])
             self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
+        if self.kind == _lib.KIND_ECLP:                    # (alpha, beta, c, s, lam, r, p) in seven weights rows
+            self.weights = torch.as_tensor(_padded(np.asarray(hp.eclp, np.float64)[spec.sel].T, self.stride, 1.0), **f64)
         if self.kind in (_lib.KIND_SUM, _lib.KIND_BINS):
             self.theta_bar = torch.zeros((2, self.stride), **f64)
         self.delta = self.lam = self.hcoef = self.hmask = None
@@ -1158,13 +1311,14 @@ class DeviceBucket:
     def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
                      W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None, sc: Optional[np.ndarray] = None,
                      rates: Optional[np.ndarray] = None, AD: Optional[np.ndarray] = None,
-                     cgam: Optional[np.ndarray] = None):
+                     cgam: Optional[np.ndarray] = None, eclp_st: Optional[np.ndarray] = None):
         """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
         Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__;
         StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,), or, when
         their A or rates change, the new rates (arity, n) in the weights rows and AD = (A, D) (2, n) in logrw rows 0-1;
         cryptoswap pools likewise, with their curve gammas cgam (n,), and AD = (A, G, D) (3, n) in logrw rows 0-2;
-        concentrated pools get their new (s, c) from sc (2, n), with R their derived reserves (ladder_state)."""
+        concentrated pools get their new (s, c) from sc (2, n), with R their derived reserves (ladder_state); E-CLPs
+        get the state (r, p) of their new reserves from eclp_st (2, n) in weights rows 5-6."""
         f64 = dict(dtype=torch.float64, device=self._device)
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
         if sc is not None:
@@ -1179,6 +1333,8 @@ class DeviceBucket:
                     self.logrw[2, li] = torch.as_tensor(cryptoswap_invariant_any(R.T, W.T, amp, cgam), **f64)
             elif self.kind == _lib.KIND_GEOMEAN:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
+        if eclp_st is not None:
+            self.weights[5:7, li] = torch.as_tensor(eclp_st, **f64)
         if rates is not None:
             self.weights[:, li] = torch.as_tensor(rates, **f64)
         if AD is not None:
@@ -1667,6 +1823,7 @@ class PoolStore:
         self._kind_host, self._weights_host = hp.kind, hp.weights      # structure: kinds, weights / bounded offsets / rates
         self._amp_host = hp.amp                                          # StableSwap / cryptoswap amplification
         self._cgam_host = hp.cgam                                        # cryptoswap curve gamma
+        self._eclp_host = hp.eclp                                        # E-CLP parameters (immutable; state on the device)
         self._own_stable = False                                         # weights / amp are this store's copies
         self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records
         self._lad = None                                                 # LadderSlab
@@ -1732,7 +1889,8 @@ class PoolStore:
         """SURVEY.md section 8(d): 32 B per 2-token pool, 28k+12 per weighted pool, 20k+24 per StableSwap pool (reserves,
         token ids, rates, gamma, A, D), 80 B per concentrated pool (token ids, gamma, (s, c, first record, T), and the b_c,
         L_c, b_{c+1} and end bound the kernel reads for a trade inside the current interval; one that crosses bounds
-        reads O(log) records more), + nu, psi, arb."""
+        reads O(log) records more), 88 B per E-CLP pool (reserves, token ids, gamma, its seven parameters and state),
+        + nu, psi, arb."""
         n = 0
         for b in self.buckets:
             n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED
@@ -1740,6 +1898,7 @@ class PoolStore:
                         else 64 if b.kind == _lib.KIND_STABLESWAP
                         else 72 if b.kind == _lib.KIND_CRYPTOSWAP
                         else 148 if b.kind == _lib.KIND_CRYPTOSWAP_3
+                        else 88 if b.kind == _lib.KIND_ECLP
                         else 20 * b.arity + 24 if b.kind == _lib.KIND_STABLESWAP_N else 32)
         return n + 16 * self.n_tokens + 8
 
@@ -1919,7 +2078,9 @@ class PoolStore:
         bucket's records like cfmm_ladder_splice: a bins= update also moves the bucket's records pointer, so a CUDA graph
         captured over this store must be captured again.  The replaced pools' multipliers (theta_bar) restart at 0, a
         fresh pool's.  A bins pool takes no reserves= (its reserves are derived from its bins).  store.bin_fills(i, t)
-        splits a trade over the pool's current bins.
+        splits a trade over the pool's current bins.  E-CLP pools take reserves= and fees=: their state (r, p) is
+        recomputed with eclp_state, as HostPools does; their parameters are structure (immutable on chain: a changed
+        pool is a new store).
 
         All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.from_lists and
         validate) raise ValueError before anything is written on the device or in the store's host state, and so does an
@@ -1974,6 +2135,11 @@ class PoolStore:
                     AD = np.stack([A, D])
                 if not bool(np.all(np.isfinite(D) & (D > 0))):
                     raise ValueError("invariant D must be finite and > 0 (scaled balances out of fp64 range?)")
+            if b.kind == _lib.KIND_ECLP and R is not None:    # the state (r, p) of the new balances, as from_lists
+                est = eclp_state(R.T, np.asarray(self._eclp_host, np.float64)[ids, :5]).T
+                if not bool(np.all(np.isfinite(est[0]) & (est[0] > 0))):
+                    raise ValueError("eclp invariant r must be finite and > 0 (balances out of fp64 range?)")
+                sc = est
             plan.append((b, loc[ids], R, g, rs, ids, sc, lad, rt, AD))
         # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
         rebuilt = 0
@@ -1989,6 +2155,9 @@ class PoolStore:
             crypto = b.kind in (_lib.KIND_CRYPTOSWAP, _lib.KIND_CRYPTOSWAP_3)
             amp_ = self._amp_host[ids] if b.kind in (_lib.KIND_STABLESWAP, _lib.KIND_STABLESWAP_N) or crypto else None
             cg_ = self._cgam_host[ids] if crypto else None
+            if b.kind == _lib.KIND_ECLP:
+                b.write_update(l, R, g, eclp_st=sc)
+                continue
             b.write_update(l, R, g, W, amp_, sc, None if u.rates is None else rt, AD, cg_)
         # the store's host state, once the device holds the update
         for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:

@@ -101,7 +101,18 @@ enum {
                               pays the smoothing term.  delta / lambda: the positive and negative parts of the flows
                               (t, -(C(t) + smoothing)).  hcoef per pool, as for every pair kind: (sigma / p_ref) r nu0
                               inside a segment, 0 at a breakpoint or an end.  cfmm_bins_update_multipliers advances
-                              tbar.                                                                                    */
+                              tbar.                                                                                    */,
+    CFMM_KIND_ECLP = 11       /* elliptic concentrated liquidity (Gyroscope E-CLP): price range 0 < alpha < beta (token 1
+                              per token 0), rotation c = cos(phi), s = sin(phi) >= 0, stretch 1 <= lam <= 1e8; with
+                              A = [[c/lam, -s/lam], [s, c]] the pool keeps ||A (t - r chi)|| <= r and t >= 0, chi =
+                              (f_x(beta), f_y(alpha)), f(p) = M (p, 1)' / sqrt((p, 1) M (p, 1)'), M = (A'A)^-1.  Its
+                              balances lie on the arc t(p) = r (chi - f(p)), p in [alpha, beta], where the marginal
+                              price is p.  Not in the reference; arity 2 (any other arity: CFMM_E_KIND).
+                              weights [7][stride] = (alpha, beta, c, s, lam, r, p): the parameters, the invariant r and
+                              the price p of the reserves (pools.eclp_state); reserves [2][stride] = (x, y), paid out
+                              exactly at a cap.  logrw is not read.  hcoef is per pool, as for every pair kind:
+                              r lam^2 nu1 p*^2 / h(p*)^3 (over gamma when tendering token 1), 0 at a cap.  Smooth: no
+                              theta_bar.  The evaluation has no TMA-staged kernel.                                     */
 };
 
 enum {
@@ -123,7 +134,8 @@ typedef struct cfmm_bucket {
     const double* reserves;
     const int32_t* tok_idx;
     const double* gamma;
-    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates; CONCENTRATED, BINS records */
+    const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates; CONCENTRATED, BINS records;
+                                ECLP (alpha, beta, c, s, lam, r, p) */
     const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D); CONCENTRATED (s, c, first record, T);
                                 BINS (first record, nb, z, p_ref) */
     const double* theta_bar; /* SUM and BINS only */
@@ -429,7 +441,7 @@ typedef struct cfmm_csr_pools {
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
     const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP |
                                             CFMM_KIND_CONCENTRATED | CFMM_KIND_CRYPTOSWAP |
-                                            CFMM_KIND_CRYPTOSWAP_3 | CFMM_KIND_BINS, else weighted
+                                            CFMM_KIND_CRYPTOSWAP_3 | CFMM_KIND_BINS | CFMM_KIND_ECLP, else weighted
                                             geometric mean                                           */
 } cfmm_csr_pools;
 
@@ -497,6 +509,14 @@ int cfmm_batch_solve_tricrypto(const cfmm_csr_pools* pools, const double* record
  * first theta_bar slot of the workspace.  A seventh kernel instance, so the others keep their registers.  Same limits
  * and workspace. */
 int cfmm_batch_solve_bins(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
+                          const cfmm_batch_params* prm, void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_ECLP pools, beside every kind cfmm_batch_solve_bins takes (the seven
+ * entry points above give their problems status 3).  In the CSR arrays an E-CLP pool carries (x, y) in its reserves and,
+ * in its first logrw slot, the index r_i of its record in `records` (units of 4 f64, as the first-record slots of
+ * concentrated and bins pools): records[4 r_i .. 4 r_i + 7] = {c, s, lam, alpha, beta, r, p, 0}, after the concentrated
+ * and bins pools' records in the same buffer (CFMM_E_NULL if NULL).  An eighth kernel instance, so the others keep their
+ * registers.  Same limits and workspace. */
+int cfmm_batch_solve_eclp(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
                           const cfmm_batch_params* prm, void* work, void* stream);
 
 /*
