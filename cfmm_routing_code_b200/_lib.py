@@ -13,6 +13,7 @@ KIND_PRODUCT, KIND_SUM, KIND_GEOMEAN, KIND_BOUNDED, KIND_STABLESWAP, KIND_STABLE
 KIND_CRYPTOSWAP, KIND_CRYPTOSWAP_3 = 8, 9
 KIND_BINS = 10
 KIND_ECLP = 11
+KIND_PMM = 12
 
 _ERRORS = {
     -1: "CFMM_E_NULL (required pointer is NULL)",
@@ -189,6 +190,8 @@ def load(build_if_missing: bool = True):
     lib.cfmm_batch_solve_bins.restype = C.c_int
     lib.cfmm_batch_solve_eclp.argtypes = lib.cfmm_batch_solve_concentrated.argtypes
     lib.cfmm_batch_solve_eclp.restype = C.c_int
+    lib.cfmm_batch_solve_pmm.argtypes = lib.cfmm_batch_solve_concentrated.argtypes
+    lib.cfmm_batch_solve_pmm.restype = C.c_int
     lib.cfmm_allreduce_ll.argtypes = [vp, vp, i32, i32, i32, i64, i64, vp, C.c_uint64, vp]
     lib.cfmm_allreduce_ll.restype = C.c_int
     lib.cfmm_sum_update_multipliers.argtypes = [C.POINTER(Bucket), vp, vp, vp, vp]

@@ -111,9 +111,11 @@ def solve(local_indices, reserves, fees, kinds, weights=None, utility=None, n_to
     HostPools.from_lists and instances.v3_ladder).  And 'cryptoswap': weights[i] = (A, gamma, p_0, p_1), a two-coin Curve v2
     (twocrypto-ng) pool with the whitepaper A, the curve's gamma and the price scales (see HostPools.from_lists and
     instances.twocrypto_pool).  And 'eclp': reserves[i] = (x, y), weights[i] = (alpha, beta, c, s, lam), a Gyroscope
-    elliptic concentrated-liquidity pool (see HostPools.from_lists and instances.eclp_pool).  Problems with StableSwap,
-    concentrated, cryptoswap or E-CLP pools run solver.py, the native host loop or the per-thread solver, never the native
-    blocked and persistent solvers."""
+    elliptic concentrated-liquidity pool (see HostPools.from_lists and instances.eclp_pool).  And 'pmm': reserves[i] =
+    (B, Q), weights[i] = (pi, k, B0, Q0), a DODO proactive market maker with its guide price, slippage factor and
+    targets (see HostPools.from_lists and instances.pmm_pool).  Problems with StableSwap, concentrated, cryptoswap, E-CLP
+    or PMM pools run solver.py, the native host loop or the per-thread solver, never the native blocked and persistent
+    solvers."""
     if utility is None:
         raise ValueError("utility is required: Arbitrage(c) | Liquidate(target, assets) | Swap(i, o, t)")
     if n_tokens is None:

@@ -15,7 +15,7 @@ import torch
 
 from . import _lib
 from .pools import HostPools, KIND_BINS_HOST, KIND_CONCENTRATED_HOST, KIND_CRYPTOSWAP_HOST, KIND_ECLP_HOST, \
-    KIND_GEOMEAN_HOST, KIND_STABLESWAP_HOST
+    KIND_GEOMEAN_HOST, KIND_PMM_HOST, KIND_STABLESWAP_HOST
 from .solver import default_nu0
 
 NTOK_MAX = 64      # cfmm_small::NTOK_MAX
@@ -94,6 +94,13 @@ class CsrStore:
             at = (len(lad) + len(bns)) // 4 + 2 * np.arange(len(ec))
             self.logrw[first] = torch.as_tensor(at.astype(np.float64), device=dev)
             self.records = torch.as_tensor(np.concatenate([lad, bns, rec.reshape(-1)]), device=dev)
+        pm = np.nonzero(np.asarray(hp.kind) == KIND_PMM_HOST)[0]
+        self.has_pmm = bool(len(pm))                 # -> cfmm_batch_solve_pmm (a ninth instance)
+        if len(pm):                                  # PMM pools: one record {pi, k, B0, Q0} each after every record
+            prev = torch.zeros(0, dtype=torch.float64, device=dev) if self.records is None else self.records   # above,
+            first = torch.as_tensor(np.asarray(hp.pool_ptr)[pm], device=dev)    # its index in the first logrw slot
+            self.logrw[first] = torch.as_tensor((prev.numel() // 4 + np.arange(len(pm))).astype(np.float64), device=dev)
+            self.records = torch.cat([prev, torch.as_tensor(np.asarray(hp.pmm, np.float64)[pm].reshape(-1), device=dev)])
         cs = np.nonzero(np.asarray(hp.kind) == KIND_CRYPTOSWAP_HOST)[0]
         ptr = np.asarray(hp.pool_ptr, np.int64)
         c3 = cs[ptr[cs + 1] - ptr[cs] == 3]
@@ -165,6 +172,10 @@ def solve_batch_device(store: CsrStore, c: torch.Tensor, a: torch.Tensor, flags:
                        store.nnz if shared else 0)
     prm = _lib.BatchParams(float(tol), 0.1, 1e-4, 0.5, 1e-12, int(max_outer), int(max_inner))
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if store.has_pmm:
+        _lib.check(store.lib.cfmm_batch_solve_pmm(C.byref(store.c_pools), store.records.data_ptr(), C.byref(batch),
+                                                  C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve_pmm")
+        return psi, stats, delta, lam
     if store.has_eclp:
         _lib.check(store.lib.cfmm_batch_solve_eclp(C.byref(store.c_pools), store.records.data_ptr(), C.byref(batch),
                                                    C.byref(prm), work.data_ptr(), st), "cfmm_batch_solve_eclp")
@@ -280,7 +291,8 @@ def pack_problems(problems: Sequence):
                        cat("cgam", np.float64), np.concatenate(bptr),
                        np.concatenate([np.asarray(hp.bin_rec, np.float64).reshape(-1, 4) for hp, _ in problems]),
                        np.concatenate([np.asarray(hp.bin_zp, np.float64).reshape(-1, 2) for hp, _ in problems]),
-                       np.concatenate([np.asarray(hp.eclp, np.float64).reshape(-1, 7) for hp, _ in problems]))
+                       np.concatenate([np.asarray(hp.eclp, np.float64).reshape(-1, 7) for hp, _ in problems]),
+                       np.concatenate([np.asarray(hp.pmm, np.float64).reshape(-1, 4) for hp, _ in problems]))
     return merged, ranges, c, a, fl, nu, nnz_max
 
 

@@ -9,7 +9,7 @@
 #include <math.h>
 
 #include "cfmm_dev.cuh"
-#include "cfmm_small.cuh"     // bounded_pair(), eclp_pair(), ladder_pair(), bins_pair(), ...: the per-pool math, shared with the per-thread solver
+#include "cfmm_small.cuh"     // bounded_pair(), eclp_pair(), pmm_pair(), ladder_pair(), bins_pair(), ...: the per-pool math, shared with the per-thread solver
 
 namespace cfmm {
 std::atomic<long long> g_launches{0};
@@ -154,6 +154,17 @@ k_eval_pair(long long m, long long ld, int n_tokens, const double* __restrict__ 
             double D[2], L[2];
             cfmm_small::eclp_pair(R0, R1, thbar[i], thbar[ld + i], thbar[2 * ld + i], thbar[3 * ld + i],
                                   thbar[4 * ld + i], thbar[5 * ld + i], thbar[6 * ld + i], g, n0, n1, D, L, h);
+            y0 = L[0] - D[0];
+            y1 = L[1] - D[1];
+            if (TRADES) {
+                delta[i] = D[0]; delta[ld + i] = D[1];
+                lambda[i] = L[0]; lambda[ld + i] = L[1];
+            }
+        } else if (KIND == CFMM_KIND_PMM) {
+            // `thbar` carries the bucket's weights [4][ld] = (pi, k, B0, Q0)
+            double D[2], L[2];
+            cfmm_small::pmm_pair(R0, R1, thbar[i], thbar[ld + i], thbar[2 * ld + i], thbar[3 * ld + i], g, n0, n1, D, L,
+                                 h);
             y0 = L[0] - D[0];
             y1 = L[1] - D[1];
             if (TRADES) {
@@ -932,8 +943,9 @@ int launch_pair(const cfmm_bucket* b, int n_tokens, const double* nu, double eps
     double* lambda = out ? out->lambda : nullptr;
     double* hcoef = out ? out->hcoef : nullptr;
     // per-slot auxiliary array: fill multipliers of constant-sum orders | virtual-reserve offsets of bounded products |
-    // the parameters and state of E-CLPs.  Neither of the last two has a TMA-staged kernel: the LDG path only.
-    constexpr bool kWeights = KIND == CFMM_KIND_BOUNDED_PRODUCT || KIND == CFMM_KIND_ECLP;
+    // the parameters and state of E-CLPs | the parameters and targets of PMMs.  None of the last three has a TMA-staged
+    // kernel: the LDG path only.
+    constexpr bool kWeights = KIND == CFMM_KIND_BOUNDED_PRODUCT || KIND == CFMM_KIND_ECLP || KIND == CFMM_KIND_PMM;
     const double* aux = kWeights ? b->weights : b->theta_bar;
     if (!kWeights && (g_scatter_mode == 0 || g_scatter_mode == 3) && tma_ok(b)) {
         auto kern = k_eval_pair_tma<kWeights ? CFMM_KIND_PRODUCT : KIND, TRADES, HESS>;
@@ -1222,6 +1234,10 @@ int validate(const cfmm_bucket* b, int n_tokens) {
             if (b->arity != 2) return CFMM_E_KIND;
             if (b->n_pools > 0 && !b->weights) return CFMM_E_NULL;       // (alpha, beta, c, s, lam, r, p)
             break;
+        case CFMM_KIND_PMM:
+            if (b->arity != 2) return CFMM_E_KIND;
+            if (b->n_pools > 0 && !b->weights) return CFMM_E_NULL;       // (pi, k, B0, Q0)
+            break;
         default:
             return CFMM_E_KIND;
     }
@@ -1259,6 +1275,8 @@ int cfmm_arb_eval(const cfmm_bucket* b, int32_t n_tokens, const double* nu, cons
             return dispatch_pair<CFMM_KIND_BINS>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_ECLP:
             return dispatch_pair<CFMM_KIND_ECLP>(b, n_tokens, nu, eps, psi, arb, out, st);
+        case CFMM_KIND_PMM:
+            return dispatch_pair<CFMM_KIND_PMM>(b, n_tokens, nu, eps, psi, arb, out, st);
         case CFMM_KIND_CRYPTOSWAP_3:
             return dispatch_crypto3(b, n_tokens, nu, psi, arb, out, st);
         case CFMM_KIND_STABLESWAP_N:

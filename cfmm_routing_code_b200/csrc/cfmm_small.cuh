@@ -174,6 +174,62 @@ CFMM_HD inline void eclp_pair(double x, double y, double alpha, double beta, dou
     }
 }
 
+// DODO proactive market maker (PMM; not a reference atom).  Guide price pi > 0 (token 1 per token 0), slippage factor
+// 0 < k <= 1, targets (B0, Q0).  Two pieces meet at (B0, Q0) with slope -pi.  Base short (b <= B0): q - Q0 = pi d (1 +
+// k d / b), d = B0 - b, marginal price pi (1 - k + k B0^2 / b^2) >= pi.  Quote short (q <= Q0): the mirror, b - B0 =
+// (e / pi)(1 + k e / q), e = Q0 - q, price pi / (1 - k + k Q0^2 / q^2) <= pi.  The reserves (B, Q) lie on the curve
+// through the adjusted-target rule (pools.pmm_targets): B < B0 (base short), Q < Q0 (quote short), or (B, Q) = (B0, Q0).
+// The end point at price p* is closed form on its piece: w = sqrt(1 + z), b* = B0 / w with z = (p* - pi) / (k pi), or
+// q* = Q0 / w with z = (pi - p*) / (k p*).  Along a piece the short token moves by |s2 - s1| and the other by the
+// integral |s2 - s1| (1 - k + k T^2 / (s1 s2)), times pi (base piece) or over pi (quote piece), never a difference of
+// two curve points; a leg from the target to s* moves T (1 - 1 / w) = T z / (w (w + 1)) (pmm_gap).
+CFMM_HD inline double pmm_gap(double T, double z, double w) { return z < 3.0 ? T * (z / (w * (w + 1.0))) : T - T / w; }
+
+// The optimal trade at prices (n0, n1) of the pool (B, Q), fee gam.  The pool's price P = pi (1 + k ((B0/B)^2 - 1))
+// on the base piece, pi / (1 + k ((Q0/Q)^2 - 1)) on the quote piece, pi at equilibrium.  Tender 0 iff p* = n0 / (gam
+// n1) < P: the price falls to p*.  Tender 1 iff p* = gam n0 / n1 > P: it rises to p*.  A trade that crosses pi runs
+// in two legs that meet at (B0, Q0).  Never a cap: b*, q* > 0 at every finite price.  hc = n1 p*^2 b* / (2 (k pi + p* -
+// pi)) for p* >= pi, n1 pi q* / (2 (k p* + pi - p*)) below, over gam when tendering 1, 0 with no trade.
+CFMM_HD inline void pmm_pair(double B, double Q, double pi, double k, double B0, double Q0, double gam, double n0,
+                             double n1, double* Dl, double* Ll, double& hc) {
+    Dl[0] = Dl[1] = Ll[0] = Ll[1] = 0.0;
+    hc = 0.0;
+    const bool bs = B < B0, qs = !bs && Q < Q0;                             // base short | quote short | equilibrium
+    const double rb = B0 / B, rq = Q0 / Q;
+    const double P = bs ? pi * fma(k, fma(rb, rb, -1.0), 1.0) : qs ? pi / fma(k, fma(rq, rq, -1.0), 1.0) : pi;
+    const double lo = n0 / (gam * n1), hi = gam * n0 / n1;
+    const bool t0 = lo < P, t1 = hi > P;
+    if (!t0 && !t1) return;
+    const double ps = t0 ? lo : hi;
+    const bool eb = ps >= pi;                                               // the trade ends on the base piece
+    const double z = eb ? (ps - pi) / (k * pi) : (pi - ps) / (k * ps);
+    const double w = sqrt(1.0 + z);
+    const double T = eb ? B0 : Q0, se = T / w;                              // the end piece's target and end point
+    double db = 0.0, dq = 0.0;                                              // token 0 and token 1 moved, >= 0
+    double s = eb ? B : Q;                                                  // where the end piece's leg starts
+    if (eb && qs) {                                                         // quote piece back to (B0, Q0) first
+        dq = Q0 - Q;
+        db = dq * fma(k, rq, 1.0 - k) / pi;
+        s = B0;
+    } else if (!eb && bs) {                                                 // base piece back to (B0, Q0) first
+        db = B0 - B;
+        dq = pi * (db * fma(k, rb, 1.0 - k));
+        s = Q0;
+    }
+    const double d = s == T ? pmm_gap(T, z, w) : fmax(t0 == eb ? se - s : s - se, 0.0);
+    const double o = d * fma(k, (T / s) * w, 1.0 - k);                      // T^2 / (s s*) = (T / s) w
+    if (eb) { db += d; dq += pi * o; } else { dq += d; db += o / pi; }
+    if (t0) {
+        Dl[0] = db / gam;
+        Ll[1] = dq;
+    } else {
+        Ll[0] = db;
+        Dl[1] = dq / gam;
+    }
+    hc = eb ? n1 * ps * se * (ps / (2.0 * fma(k, pi, ps - pi))) : n1 * pi * se / (2.0 * fma(k, ps, pi - ps));
+    if (t1) hc /= gam;
+}
+
 // Concentrated-liquidity pool (a whole Uniswap-v3 tick ladder): sqrt-price bounds b_0 < ... < b_T, liquidity L_k on
 // [b_k, b_{k+1}), current sqrt price s in [b_0, b_T] inside interval c (b_c <= s, c <= T - 1).  One record per bound,
 // rec[4k .. 4k+3] = {b_k, L_k, Y_k, X_k}: Y_k = sum_{j<k} L_j (b_{j+1} - b_j) (token 1 below b_k), X_k =
@@ -1052,8 +1108,11 @@ CFMM_UNROLL
 // ECLP (with all six): also E-CLP pools (kind 11) through eclp_pair, their record {c, s, lam, alpha, beta, r, p, 0} (two
 // record slots) in `rec` after the ladders' and bins', its record index in the pool's first logrw slot;
 // cfmm_batch_solve_eclp runs this eighth instance.  The others give such problems status 3.
+// PMM (with all seven): also DODO PMM pools (kind 12) through pmm_pair, their record {pi, k, B0, Q0} (one record slot)
+// in `rec` after the E-CLPs', its record index in the pool's first logrw slot; cfmm_batch_solve_pmm runs this ninth
+// instance.  The others give such problems status 3.
 template <int LANES, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
-          bool CRYPTO3 = false, bool BINS = false, bool ECLP = false>
+          bool CRYPTO3 = false, bool BINS = false, bool ECLP = false, bool PMM = false>
 CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, const Vec& lognu, double eps,
                                const Vec& psi, const Vec* Hs, bool trades, bool store_fill, int lane,
                                const double* rec = nullptr) {
@@ -1137,6 +1196,15 @@ CFMM_HD inline double evaluate(const Pools& P, const Problem& Q, const Vec& nu, 
             const double* e = rec + 4 * (int64_t)P.logrw[off];
             eclp_pair(P.R[off], P.R[off + 1], e[3], e[4], e[0], e[1], e[2], e[5], e[6], gam, nu[P.tok[off]],
                       nu[P.tok[off + 1]], D, L, hc);
+            if (Hs && hc != 0.0) {
+                const int t0 = P.tok[off], t1 = P.tok[off + 1];
+                (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
+                (*Hs)[t0 * n + t1] -= hc; (*Hs)[t1 * n + t0] -= hc;
+            }
+        } else if (PMM && P.kind[i] == 12) {                          // {pi, k, B0, Q0} in rec
+            double hc = 0.0;
+            const double* e = rec + 4 * (int64_t)P.logrw[off];
+            pmm_pair(P.R[off], P.R[off + 1], e[0], e[1], e[2], e[3], gam, nu[P.tok[off]], nu[P.tok[off + 1]], D, L, hc);
             if (Hs && hc != 0.0) {
                 const int t0 = P.tok[off], t1 = P.tok[off + 1];
                 (*Hs)[t0 * n + t0] += hc; (*Hs)[t1 * n + t1] += hc;
@@ -1342,7 +1410,7 @@ CFMM_HD inline int64_t work_doubles(int n, int64_t nnz) { return 12LL * n + 2LL 
 // The solve.  nu_io [n]: start prices in, optimal prices out.  psi_out [n].  `work`/`stride`: interleaved workspace.
 // rec: the concentrated and price-bin pools' records (LADDER and BINS instances only).
 template <int LANES = 1, bool STABLE = false, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false,
-          bool CRYPTO3 = false, bool BINS = false, bool ECLP = false>
+          bool CRYPTO3 = false, bool BINS = false, bool ECLP = false, bool PMM = false>
 CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, double* nu_io, double* psi_out,
                                double* work, int64_t stride, int lane = 0, const double* rec = nullptr) {
     const int n = Q.n;
@@ -1363,10 +1431,11 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         const int k = (int)(P.pool_ptr[i + 1] - o);
         has_sum = has_sum || P.kind[i] == 1 || (BINS && P.kind[i] == 10);
         bad = (P.kind[i] > (STABLE ? 4 : 3) && !(LADDER && P.kind[i] == 6) && !(CRYPTO && P.kind[i] == 8) &&
-               !(CRYPTO3 && P.kind[i] == 9) && !(BINS && P.kind[i] == 10) && !(ECLP && P.kind[i] == 11)) || k < 2 ||
+               !(CRYPTO3 && P.kind[i] == 9) && !(BINS && P.kind[i] == 10) && !(ECLP && P.kind[i] == 11) &&
+               !(PMM && P.kind[i] == 12)) || k < 2 ||
               k > KMAX || ((P.kind[i] == 1 || P.kind[i] == 3 || (STABLE && !STABLE_N && P.kind[i] == 4) ||
                 (LADDER && P.kind[i] == 6) || (CRYPTO && P.kind[i] == 8) || (BINS && P.kind[i] == 10) ||
-                (ECLP && P.kind[i] == 11)) && k != 2) ||
+                (ECLP && P.kind[i] == 11) || (PMM && P.kind[i] == 12)) && k != 2) ||
               (CRYPTO3 && P.kind[i] == 9 && k != 3);
         for (int j = 0; j < k && !bad; ++j) bad = P.tok[o + j] < 0 || P.tok[o + j] >= n;
     }
@@ -1394,7 +1463,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
     uint64_t free_mask = 0, fm_t = 0;
 
     for (int outer = 0; outer < prm.max_outer; ++outer) {
-        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
+        g = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(P, Q, nuv[cur], lognu, eps_t, psiv[cur], &Hsv[cur], false, false, lane, rec));
         ++evals;
         int inner_status = 1;
         const double inner_tol = has_sum ? fmax(prm.tol, fmin(1e-3, 1e-2 * move)) : prm.tol;
@@ -1440,7 +1509,7 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
                         nuv[nxt][j] = v;
                         lin += grad[j] * (v - nuv[cur][j]);
                     }
-                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
+                    g_t = dual_value(Q, nuv[nxt], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(P, Q, nuv[nxt], lognu, eps_t, psiv[nxt], &Hsv[nxt], false, false, lane, rec));
                     ++evals;
                     if (ls == 0) lin1 = lin;
                     if (g_t <= g + 1e-4 * lin) { ok = true; break; }
@@ -1465,8 +1534,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
         }
         if (!has_sum) { status = inner_status; break; }
         // exact duality gap at the current prices (trades from the smoothed problem, dual with eps = 0)
-        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
-        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+        evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(P, Q, nuv[cur], lognu, eps_t, psiv[cur ^ 1], nullptr, false, true, lane, rec);
+        const double g_exact = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
         evals += 2;
         double primal = 0.0;
         for (int j = 0; j < n; ++j) primal += Q.c[j] * psiv[cur ^ 1][j];
@@ -1499,8 +1568,8 @@ CFMM_HD inline Stats solve_one(const Pools& P, Problem Q, const Params& prm, dou
 
     // final read-out: trades and psi from the (smoothed) problem, dual value from the exact one
     const Vec& psi_f = psiv[cur ^ 1];
-    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
-    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
+    evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(P, Q, nuv[cur], lognu, eps_t, psi_f, nullptr, true, false, lane, rec);
+    const double dval = dual_value(Q, nuv[cur], evaluate<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(P, Q, nuv[cur], lognu, 0.0, grad_t, nullptr, false, false, lane, rec));
     evals += 2;
     double primal = 0.0, viol = 0.0;
     for (int j = 0; j < n; ++j) {

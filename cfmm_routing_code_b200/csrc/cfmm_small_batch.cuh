@@ -24,9 +24,9 @@ constexpr int kSmallThreads = 32;     // one warp per CTA: a sweep of 50 problem
 // STABLE_N: StableSwap pools of 2..8 coins (k_batch_solve_stable_n).  LADDER: concentrated pools too, their records in
 // `rec` (k_batch_solve_ladder).  CRYPTO: two-coin cryptoswap pools too (k_batch_solve_crypto).  CRYPTO3: three-coin
 // cryptoswap pools too (k_batch_solve_tricrypto).  BINS: price-bin pools too (k_batch_solve_bins).  ECLP: E-CLP pools
-// too (k_batch_solve_eclp).
+// too (k_batch_solve_eclp).  PMM: DODO PMM pools too (k_batch_solve_pmm).
 template <int LANES, bool STABLE, bool STABLE_N = false, bool LADDER = false, bool CRYPTO = false, bool CRYPTO3 = false,
-          bool BINS = false, bool ECLP = false>
+          bool BINS = false, bool ECLP = false, bool PMM = false>
 __device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, const cfmm_batch& B, const cfmm_small::Params& prm,
                                                  int n, long long n_pools, double* work, long long stride,
                                                  const double* rec = nullptr) {
@@ -52,7 +52,7 @@ __device__ __forceinline__ void batch_solve_body(const cfmm_small::Pools& P, con
     Q.flags = B.flags + p * n;
     Q.delta = B.delta ? B.delta + p * B.trade_stride : nullptr;
     Q.lam = B.lambda ? B.lambda + p * B.trade_stride : nullptr;
-    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP>(
+    const cfmm_small::Stats r = cfmm_small::solve_one<LANES, STABLE, STABLE_N, LADDER, CRYPTO, CRYPTO3, BINS, ECLP, PMM>(
         P, Q, prm, B.nu + p * n, B.psi + p * n, work + (LANES == 1 ? p : p * LANES + lane), stride, lane, rec);
     if (lane == 0) {
         st[0] = r.value; st[1] = r.dual; st[2] = r.gap; st[3] = r.infeas; st[4] = r.err;

@@ -592,6 +592,89 @@ def synth_eclp_market(m, n_tokens, seed, frac_eclp=0.3, lam=(1.0, 1e4), misprici
     return hp, p
 
 
+def pmm_pool(reserves, targets, r_state, i, K, lp_fee_rate, mt_fee_rate, decimals):
+    """A DODO v2 PMM pool's raw on-chain state as ("pmm" reserves, weights, gamma).  reserves = the raw base and quote
+    reserves (_BASE_RESERVE_, _QUOTE_RESERVE_), targets = the stored raw targets (_BASE_TARGET_, _QUOTE_TARGET_),
+    r_state = _RState_ (0 ONE, 1 ABOVE_ONE: base short, 2 BELOW_ONE: quote short), i = _I_ and K = _K_ (18 decimals; i
+    in raw quote per raw base), the 18-decimal LP and maintainer fee rates, decimals = the (base, quote) token decimals.
+
+    The contracts' adjusted-target rule decides the short side by r_state and re-derives its target from the reserves
+    and the long side's stored target (pools.pmm_targets, which HostPools.from_lists applies again and leaves as it
+    is).  At ONE the pool is taken at its reserves, (B0, Q0) = (B, Q): the contracts keep trading from the stored
+    targets there and leave any excess of the reserves over them aside, so the model is deeper by that excess.  DODO
+    charges its fees on the output; gamma = 1 - (lpFeeRate + mtFeeRate) charges them on the input instead, the same
+    approximation as twocrypto_pool (exact to first order in the fee).  A long side whose stored target is 0 (a DVM,
+    which prices from a quote target of 0, so its curve ends at price i) raises ValueError: that curve has a cap.
+    Agreement with the contracts' fixed-point arithmetic is not verified (INTEGRATION.md)."""
+    from decimal import Decimal, localcontext
+    from .pools import pmm_targets
+    bd, qd = int(decimals[0]), int(decimals[1])
+    with localcontext() as ctx:
+        ctx.prec = 50
+        B, Q = float(Decimal(int(reserves[0])) / Decimal(10) ** bd), float(Decimal(int(reserves[1])) / Decimal(10) ** qd)
+        B0, Q0 = float(Decimal(int(targets[0])) / Decimal(10) ** bd), float(Decimal(int(targets[1])) / Decimal(10) ** qd)
+        pi = float(Decimal(int(i)) / Decimal(10) ** 18 * Decimal(10) ** (bd - qd))
+        k = float(Decimal(int(K)) / Decimal(10) ** 18)
+        gamma = float(1 - (Decimal(int(lp_fee_rate)) + Decimal(int(mt_fee_rate))) / Decimal(10) ** 18)
+    rs = int(r_state)
+    if rs not in (0, 1, 2):
+        raise ValueError("r_state must be 0 (ONE), 1 (ABOVE_ONE) or 2 (BELOW_ONE)")
+    if (rs == 1 and not Q0 > 0) or (rs == 2 and not B0 > 0):
+        raise ValueError("pmm: the long side's target is 0 (a DVM prices from a quote target of 0): the curve ends at "
+                         "price i, a cap the pmm kind does not model")
+    if not (B > 0 and Q > 0):
+        raise ValueError("pmm: both reserves must be > 0")
+    if rs == 1 and Q < Q0:
+        raise ValueError("pmm: ABOVE_ONE (base short) with the quote reserve below its target")
+    if rs == 2 and B < B0:
+        raise ValueError("pmm: BELOW_ONE (quote short) with the base reserve below its target")
+    # the short side's given target just above its reserve, so that pmm_targets re-derives it from the long side's
+    given = [(B, Q), (np.nextafter(B, np.inf), Q0), (B0, np.nextafter(Q, np.inf))][rs]
+    w = pmm_targets([[B, Q]], [[pi, k, given[0], given[1]]])[0]
+    return [B, Q], tuple(float(v) for v in w), gamma
+
+
+def synth_pmm_market(m, n_tokens, seed, frac_pmm=0.3, mispricing=0.02):
+    """A market of DODO PMM pools beside every other kind: a frac_pmm share of m pools are PMM pools on random token
+    pairs, their guide price pi at the market price (off by `mispricing`), k log-uniform over [PMM_K_MIN, 1], targets
+    whose values differ by up to e either way, fees 0.01 .. 0.3 %; a third of them at equilibrium, a third base short and
+    a third quote short, with the pool's price within `mispricing` of pi; the rest is synth_eclp_market's mix (every
+    other kind but bins).  n_tokens >= 3.  Returns (HostPools, prices)."""
+    from .pools import HostPools, KIND_PMM_HOST, PMM_K_MIN, pmm_targets
+    rng = np.random.default_rng(seed + 104729)
+    n_p = int(round(frac_pmm * m))
+    base, p = synth_eclp_market(m - n_p, n_tokens, seed, mispricing=mispricing)
+    a = rng.integers(0, n_tokens, n_p)
+    b = (a + rng.integers(1, n_tokens, n_p)) % n_tokens
+    pi = p[a] / p[b] * np.exp(mispricing * rng.standard_normal(n_p))       # token b per token a
+    k = np.exp(rng.uniform(np.log(PMM_K_MIN), 0.0, n_p))
+    Q0 = np.exp(9.0 + 1.5 * rng.standard_normal(n_p)) / p[b]
+    B0 = Q0 / pi * np.exp(rng.uniform(-1.0, 1.0, n_p))
+    side = rng.integers(0, 3, n_p)                                          # 0 equilibrium, 1 base short, 2 quote short
+    off = np.exp(np.abs(mispricing * rng.standard_normal(n_p)))             # the pool's price over (or under) pi
+    Bs = B0 * np.sqrt(k / (off - 1.0 + k))                                  # P = pi off on the base piece
+    Qs = Q0 * np.sqrt(k / (off - 1.0 + k))                                  # P = pi / off on the quote piece
+    B = np.where(side == 1, Bs, B0)
+    Q = np.where(side == 2, Qs, Q0)
+    Q = np.where(side == 1, Q0 + pi * (B0 - B) * (1.0 + k * (B0 - B) / B), Q)
+    B = np.where(side == 2, B0 + (Q0 - Q) * (1.0 + k * (Q0 - Q) / Q) / pi, B)
+    R = np.stack([B, Q], axis=1)
+    W = pmm_targets(R, np.stack([pi, k, np.where(side == 1, np.maximum(B0, np.nextafter(B, np.inf)), B0),
+                                 np.where(side == 2, np.maximum(Q0, np.nextafter(Q, np.inf)), Q0)], axis=1))
+    gam = np.array([0.9999, 0.9995, 0.999, 0.997])[rng.integers(0, 4, n_p)]
+    z2 = lambda k: np.zeros((n_p, k))
+    hp = HostPools(n_tokens, np.concatenate([base.pool_ptr, base.pool_ptr[-1] + 2 * np.arange(1, n_p + 1)]).astype(np.int64),
+                   np.concatenate([base.tok_idx, np.stack([a, b], 1).ravel()]).astype(np.int32),
+                   np.concatenate([base.reserves, R.ravel()]), np.concatenate([base.weights, np.zeros(2 * n_p)]),
+                   np.concatenate([base.gamma, gam]),
+                   np.concatenate([base.kind, np.full(n_p, KIND_PMM_HOST, np.uint8)]).astype(np.uint8),
+                   np.concatenate([base.amp, np.zeros(n_p)]), np.concatenate([base.inv, np.zeros(n_p)]),
+                   np.concatenate([base.lad_ptr, np.full(n_p, base.lad_ptr[-1], np.int64)]), base.lad_rec,
+                   np.concatenate([base.lad_sc, z2(2)]), np.concatenate([np.asarray(base.cgam, float), np.zeros(n_p)]),
+                   eclp=np.concatenate([base.eclp, z2(7)]), pmm=np.concatenate([np.zeros((base.m, 4)), W]))
+    return hp, p
+
+
 LB_ID_OFFSET = 1 << 23      # Liquidity Book's bin id of price 1 (raw units)
 
 

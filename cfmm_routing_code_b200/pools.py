@@ -32,6 +32,8 @@ LADDER_T_MAX = 1 << 20  # most intervals of one concentrated pool (cfmm_small::L
 BINS_K_MAX = 1 << 20    # most bins of one price-bin pool (cfmm_small::BINS_K_MAX)
 KIND_ECLP_HOST = 11     # elliptic concentrated liquidity (Gyroscope E-CLP); (alpha, beta, c, s, lam, r, p) in HostPools.eclp
 ECLP_LAM_MAX = 1e8      # largest stretch lam of an E-CLP
+KIND_PMM_HOST = 12      # DODO proactive market maker (PMM); (pi, k, B0, Q0) in HostPools.pmm
+PMM_K_MIN = 1e-6        # smallest slippage factor k of a PMM pool (k = 0 is a constant-price pool with caps)
 
 
 def _two_prod(a, b):
@@ -121,6 +123,93 @@ def _check_eclp(params, reserves, where=""):
         raise ValueError(f"{where}eclp reserves must be finite, >= 0 and not both 0")
     h = np.hypot(c, s)
     P[:, 2], P[:, 3] = c / h, s / h
+    return P
+
+
+def _two_sum(a, b):
+    """a + b = s + e exactly (Knuth)"""
+    s = a + b
+    bb = s - a
+    return s, (a - (s - bb)) + (b - bb)
+
+
+def _dd_mul(x, y):
+    """the double-double product of (hi, lo) pairs, to about 2^-104 relative"""
+    p, e = _two_prod(x[0], y[0])
+    return _two_sum(p, e + (x[0] * y[1] + x[1] * y[0]))
+
+
+def _dd_add(x, y):
+    s, e = _two_sum(x[0], y[0])
+    return _two_sum(s, e + (x[1] + y[1]))
+
+
+def _pmm_over(T, S, L, L0, a, c, k):
+    """whether the curve of short-side target T passes above the reserves (S short, L long, L0 its target): the sign of
+    a d S + a k d^2 - (L - L0) c S, d = T - S, in double-double arithmetic (IEEE double operations only, so the same on
+    every host).  Base short: (a, c) = (pi, 1), the curve's excess pi d (1 + k d / S) - (L - L0) times S; quote short:
+    (a, c) = (1, pi), its mirror times pi S."""
+    z = np.zeros_like(S)
+    d = _two_sum(T, -S)
+    t = _dd_add(_dd_mul(_dd_mul((a, z), d), (S, z)), _dd_mul(_dd_mul(_two_prod(a, k), d), d))
+    r = _dd_mul(_dd_mul(_two_sum(L, -L0), (c, z)), (S, z))
+    g = _dd_add(t, (-r[0], -r[1]))
+    return (g[0] > 0) | ((g[0] == 0) & (g[1] > 0))
+
+
+def pmm_targets(reserves, params) -> np.ndarray:
+    """The adjusted-target rule of DODO PMM pools: reserves [m, 2] = (B, Q), params [m, 4] = (pi, k, B0, Q0).  The
+    long side's target is kept and the short side's re-derived so that (B, Q) lies on the curve: base short (B < B0,
+    Q >= Q0), B0 = B + 2 (Q - Q0) / (pi (1 + sqrt(1 + 4 k (Q - Q0) / (pi B)))), the root of the curve's quadratic in a
+    form without cancellation; quote short (Q < Q0, B >= B0), its mirror Q0 = Q + 2 pi (B - B0) / (1 + sqrt(1 + 4 k pi
+    (B - B0) / Q)); neither short, (B0, Q0) = (B, Q), and so is a short side whose re-derived target rounds to its
+    reserve.  The re-derived target is then stepped down an ulp at a time until the curve it defines passes on or below
+    the reserves (the residual in double-double arithmetic, _pmm_over): the pool prices from the short coordinate, so a target rounded
+    up would leave it below its curve by up to an ulp of the long side's target, and a trade across pi would carry that
+    out to p*.  Both short is not a state of the pool: ValueError.  Returns [m, 4] (pi, k, B0, Q0); idempotent."""
+    R = np.asarray(reserves, np.float64).reshape(-1, 2)
+    P = np.array(params, np.float64).reshape(-1, 4)
+    B, Q = R[:, 0], R[:, 1]
+    pi, k, B0, Q0 = (P[:, j] for j in range(4))
+    if bool(np.any((B < B0) & (Q < Q0))):
+        raise ValueError("pmm: both reserves below their targets (B < B0 and Q < Q0) is not a state of the pool")
+    bs, qs = (B < B0) & (Q >= Q0), (Q < Q0) & (B >= B0)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        dq, db = np.where(bs, Q - Q0, 0.0), np.where(qs, B - B0, 0.0)
+        nb0 = np.where(bs, B + 2.0 * dq / (pi * (1.0 + np.sqrt(1.0 + 4.0 * k * dq / (pi * B)))), B)
+        nq0 = np.where(qs, Q + 2.0 * pi * db / (1.0 + np.sqrt(1.0 + 4.0 * k * pi * db / Q)), Q)
+        one = np.ones_like(B)
+        for _ in range(16):                               # the formula is within a few ulp: a few steps at most
+            hb = bs & (nb0 > B) & _pmm_over(nb0, B, Q, Q0, pi, one, k)
+            hq = qs & (nq0 > Q) & _pmm_over(nq0, Q, B, B0, one, pi, k)
+            if not (hb.any() or hq.any()):
+                break
+            nb0 = np.where(hb, np.nextafter(nb0, 0.0), nb0)
+            nq0 = np.where(hq, np.nextafter(nq0, 0.0), nq0)
+    eq = ~((bs & (nb0 > B)) | (qs & (nq0 > Q)))           # at the meeting point, or a re-derived target at its reserve
+    P[:, 2] = np.where(eq, B, np.where(bs, nb0, B0))
+    P[:, 3] = np.where(eq, Q, np.where(qs, nq0, Q0))
+    return P
+
+
+def _check_pmm(params, reserves, where=""):
+    """The value rules of PMM pools: pi finite and > 0, PMM_K_MIN <= k <= 1, targets B0, Q0 finite and > 0, reserves
+    finite and > 0.  Returns params [m, 4]."""
+    P = np.array(params, np.float64).reshape(-1, 4)
+    R = np.asarray(reserves, np.float64).reshape(-1, 2)
+    if not bool(np.all(np.isfinite(P))):
+        raise ValueError(f"{where}pmm parameters (pi, k, B0, Q0) must be finite")
+    if not bool(np.all(P[:, 0] > 0)):
+        raise ValueError(f"{where}pmm guide price pi must be > 0")
+    if bool(np.any(P[:, 1] == 0)):
+        raise ValueError(f"{where}pmm k = 0 is a constant-price pool whose trades stop at its reserves (caps); it is "
+                         f"not supported: k must lie in [{PMM_K_MIN:g}, 1]")
+    if not bool(np.all((P[:, 1] >= PMM_K_MIN) & (P[:, 1] <= 1))):
+        raise ValueError(f"{where}pmm slippage factor k must lie in [{PMM_K_MIN:g}, 1]")
+    if not bool(np.all((P[:, 2] > 0) & (P[:, 3] > 0))):
+        raise ValueError(f"{where}pmm targets B0, Q0 must be > 0")
+    if not bool(np.all(np.isfinite(R) & (R > 0))):
+        raise ValueError(f"{where}pmm reserves (B, Q) must be finite and > 0")
     return P
 
 
@@ -585,9 +674,14 @@ class HostPools:
     # E-CLP pools (kind 11): eclp[i] = (alpha, beta, c, s, lam, r, p), the parameters with (c, s) normalised and the state
     # of the reserves (eclp_state); 0 on other kinds.  Their weights are 0.  None: no E-CLP pools.
     eclp: Optional[np.ndarray] = None      # f64 [m, 7]
+    # DODO PMM pools (kind 12): pmm[i] = (pi, k, B0, Q0), the guide price, the slippage factor and the targets with the
+    # short side's re-derived (pmm_targets); 0 on other kinds.  Their weights are 0.  None: no PMM pools.
+    pmm: Optional[np.ndarray] = None       # f64 [m, 4]
 
     def __post_init__(self):
         m = len(self.gamma)
+        if self.pmm is None:
+            self.pmm = np.zeros((m, 4))
         if self.eclp is None:
             self.eclp = np.zeros((m, 7))
         if self.bin_ptr is None:
@@ -643,7 +737,11 @@ class HostPools:
         concentrated-liquidity pool, Gyroscope E-CLP): reserves[i] = (x, y), finite, >= 0, not both 0; weights[i] =
         (alpha, beta, c, s, lam) with the price range 0 < alpha < beta in token 1 per token 0, c = cos(phi), s = sin(phi)
         >= 0 (|c^2 + s^2 - 1| <= 1e-12; normalised here), 1 <= lam <= ECLP_LAM_MAX; the state (r, p) comes from
-        eclp_state.  instances.eclp_pool converts a pool's on-chain state."""
+        eclp_state.  instances.eclp_pool converts a pool's on-chain state.  And 'pmm' (a DODO v2 proactive market
+        maker, DSP or DPP; a DVM's quote target of 0 is a cap this kind does not model): reserves[i] = (B, Q), the base (token 0) and quote (token 1) balances, finite and > 0; weights[i]
+        = (pi, k, B0, Q0) with the guide price pi > 0 (token 1 per token 0), the slippage factor PMM_K_MIN <= k <= 1 and
+        the targets B0, Q0 > 0; the short side's target is re-derived from the reserves (pmm_targets), both sides short
+        raises.  instances.pmm_pool converts a pool's on-chain state."""
         m = len(local_indices)
         if not (len(reserves) == len(fees) == len(kinds) == m):
             raise ValueError("local_indices, reserves, fees, kinds must have one entry per pool")
@@ -653,8 +751,20 @@ class HostPools:
         lad = {}                                         # concentrated pool -> its records and price
         bins = {}                                        # bins pool -> bin_records
         ecl = {}                                         # E-CLP pool -> its checked parameters
+        pmm = {}                                         # PMM pool -> its checked parameters
         for i, l in enumerate(local_indices):
             k = len(l)
+            if kinds[i] == "pmm":
+                if k != 2 or len(set(int(t) for t in l)) != 2:
+                    raise ValueError(f"pool {i}: pmm pools need 2 distinct tokens")
+                if reserves[i] is None or len(reserves[i]) != 2:
+                    raise ValueError(f"pool {i}: pmm needs reserves[i] = (B, Q)")
+                if weights is None or weights[i] is None or len(weights[i]) != 4:
+                    raise ValueError(f"pool {i}: pmm needs weights[i] = (pi, k, B0, Q0)")
+                pmm[i] = _check_pmm(weights[i], reserves[i], f"pool {i}: ")[0]
+                ptr.append(ptr[-1] + 2); idx += [int(t) for t in l]; res += [float(x) for x in reserves[i]]
+                wts += [0.0, 0.0]; kd.append(KIND_PMM_HOST)
+                continue
             if kinds[i] == "eclp":
                 if k != 2 or len(set(int(t) for t in l)) != 2:
                     raise ValueError(f"pool {i}: eclp pools need 2 distinct tokens")
@@ -755,10 +865,20 @@ class HostPools:
             first = np.asarray(ptr, np.int64)[ids]
             eclp[ids, :5] = np.stack([ecl[i] for i in ids.tolist()])
             eclp[ids, 5:] = eclp_state(np.stack([res[first], res[first + 1]], axis=1), eclp[ids, :5])
+        pm = np.zeros((m, 4))
+        if pmm:
+            ids = np.asarray(sorted(pmm), np.int64)
+            first = np.asarray(ptr, np.int64)[ids]
+            Pm, Rm = np.stack([pmm[i] for i in ids.tolist()]), np.stack([res[first], res[first + 1]], axis=1)
+            short = (Rm[:, 0] < Pm[:, 2]) & (Rm[:, 1] < Pm[:, 3])
+            if short.any():
+                raise ValueError(f"pool {int(ids[short][0])}: pmm: both reserves below their targets (B < B0 and "
+                                 f"Q < Q0) is not a state of the pool")
+            pm[ids] = pmm_targets(Rm, Pm)
         return HostPools(int(n_tokens), np.asarray(ptr, np.int64), np.asarray(idx, np.int32),
                          res, np.asarray(wts, np.float64),
                          np.asarray(fees, np.float64), np.asarray(kd, np.uint8), amp, None, lad_ptr,
-                         np.concatenate(recs) if recs else None, lad_sc, cgam, bin_ptr, brec, bin_zp, eclp)
+                         np.concatenate(recs) if recs else None, lad_sc, cgam, bin_ptr, brec, bin_zp, eclp, pm)
 
     @staticmethod
     def from_pairs(n_tokens, idx, reserves, gamma) -> "HostPools":
@@ -795,6 +915,7 @@ class HostPools:
         self._validate_ladders()
         self._validate_bins()
         self._validate_eclp()
+        self._validate_pmm()
         if np.any(self.gamma <= 0) or np.any(self.gamma > 1):
             raise ValueError("fees (gamma) must lie in (0, 1]")
         if self.tok_idx.min(initial=0) < 0 or self.tok_idx.max(initial=0) >= self.n_tokens:
@@ -835,6 +956,24 @@ class HostPools:
         r, p = E[ids, 5], E[ids, 6]
         if not bool(np.all(np.isfinite(r) & (r > 0) & (p >= E[ids, 0]) & (p <= E[ids, 1]))):
             raise ValueError("eclp state (r, p): r finite and > 0, p in [alpha, beta] (eclp_state)")
+
+    def _validate_pmm(self):
+        """The rules of PMM pools on the CSR form: arity 2, the value rules of _check_pmm, and targets that the
+        adjusted-target rule leaves as they are (pmm_targets of the reserves and targets returns them bit for bit)."""
+        pm = np.asarray(self.kind) == KIND_PMM_HOST
+        P = np.asarray(self.pmm, np.float64)
+        if P.shape != (self.m, 4):
+            raise ValueError("pmm must be an [m, 4] array")
+        if not pm.any():
+            return
+        ids = np.nonzero(pm)[0]
+        if np.any(np.diff(self.pool_ptr)[ids] != 2):
+            raise ValueError("pmm pools must have 2 tokens")
+        first = np.asarray(self.pool_ptr, np.int64)[ids]
+        R = np.stack([self.reserves[first], self.reserves[first + 1]], axis=1)
+        _check_pmm(P[ids], R)
+        if not np.array_equal(pmm_targets(R, P[ids]), P[ids]):
+            raise ValueError("pmm targets (B0, Q0) must follow the adjusted-target rule of the reserves (pmm_targets)")
 
     def _validate_bins(self):
         """The rules of price-bin pools on the CSR form: arity 2; 2 .. BINS_K_MAX + 2 records, none on other kinds; T
@@ -945,6 +1084,7 @@ class PoolUpdate:
     rates: Optional[np.ndarray] = None    # f64 [nnz] new rates (price scales) of StableSwap (cryptoswap) pools at `slots`
     curve_gamma: Optional[np.ndarray] = None   # f64 [n] new curve gammas of cryptoswap pools, or None
     bins: Optional[list] = None           # [n] bin_records of the new (prices, x, y) of price-bin pools, or None
+    pmm: Optional[np.ndarray] = None      # f64 [n, 4] new (pi, k, B0, Q0) of PMM pools as given, or None
 
 
 def _pool_rows(vals, n, ar, what):
@@ -963,7 +1103,7 @@ def _pool_rows(vals, n, ar, what):
 
 def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarray, pool_ids, reserves=None,
                       fees=None, prices=None, ladders=None, amp=None, rates=None, curve_gamma=None,
-                      bins=None) -> PoolUpdate:
+                      bins=None, pmm=None) -> PoolUpdate:
     """Host checks of PoolStore.update_pools, on the problem's CSR arrays (pool_ptr, kind, weights as in HostPools).
     pool_ids: global pool indices, distinct and in range; reserves[k]: the new reserve vector of pool pool_ids[k] with the
     pool's arity (a row of the reference's `reserves` literal; an (n, k) array when all pools have arity k); fees[k]: its
@@ -977,7 +1117,9 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
     pools only); amp= and rates= may not mix StableSwap and cryptoswap pools in one call.  bins[k]: the new
     (prices, x, y) of price-bin pool pool_ids[k], the triple of HostPools.from_lists' weights[i] (K may differ from the
     pool's old K; the rules of from_lists, and records finite as bin_records checks); a bins pool takes no reserves=.
-    Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order and the
+    pmm[k]: the new (pi, k, B0, Q0) of PMM pool pool_ids[k] (an (n, 4) array or a list), under the rules of from_lists;
+    with reserves= too, the target rule is applied to both here (both sides short raises), otherwise by update_pools on
+    the pool's current reserves.  Raises ValueError; returns the update with the reserves and rates flattened into the pools' CSR slot order and the
     new bins as their bin_records."""
     m = len(pool_ptr) - 1
     ids = np.asarray(pool_ids)
@@ -985,9 +1127,9 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
         raise ValueError("pool_ids must be a 1-d sequence of integer pool indices")
     ids = ids.astype(np.int64)
     n = len(ids)
-    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates, curve_gamma, bins)):
-        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates, curve_gamma, bins or "
-                         "several")
+    if all(x is None for x in (reserves, fees, prices, ladders, amp, rates, curve_gamma, bins, pmm)):
+        raise ValueError("nothing to update: give reserves, fees, prices, ladders, amp, rates, curve_gamma, bins, pmm "
+                         "or several")
     if n and (ids.min() < 0 or ids.max() >= m):
         raise ValueError(f"pool id out of range [0, {m})")
     if reserves is not None and bool(np.any(np.asarray(kind)[ids] == KIND_BINS_HOST)):
@@ -1099,7 +1241,21 @@ def check_pool_update(pool_ptr: np.ndarray, kind: np.ndarray, weights: np.ndarra
             _check_stableswap(np.ones(len(sel)) if A is None else A[sel],
                               np.ones((len(sel), k)) if W is None else W[first[sel][:, None] + np.arange(k)],
                               np.ones((len(sel), k)))
-    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W, CG, brec)
+    PM = None
+    if pmm is not None:
+        if len(pmm) != n:
+            raise ValueError("pmm: one (pi, k, B0, Q0) per pool")
+        if not bool(np.all(np.asarray(kind)[ids] == KIND_PMM_HOST)):
+            raise ValueError("pmm= applies to pmm pools only")
+        rows = [np.asarray(r, np.float64).reshape(-1) for r in pmm]
+        if any(len(r) != 4 for r in rows):
+            raise ValueError("pmm: each entry is (pi, k, B0, Q0)")
+        PM = np.stack(rows) if rows else np.zeros((0, 4))
+        Rp = np.ones((n, 2)) if R is None else R.reshape(-1, 2)
+        _check_pmm(PM, Rp, "pmm: ")
+        if R is not None:
+            pmm_targets(Rp, PM)                           # both sides short raises
+    return PoolUpdate(ids, first, slots, R, g, pr, lad, A, W, CG, brec, PM)
 
 
 class BucketSpec:
@@ -1193,6 +1349,11 @@ def split_buckets(hp: HostPools, rank: int = 0, world: int = 1) -> List["BucketS
         if np.any(ar[ec] != 2):
             raise ValueError("eclp pools must have 2 tokens")
         keys.append((_lib.KIND_ECLP, 2, np.nonzero(ec)[0]))
+    pm = hp.kind == KIND_PMM_HOST
+    if pm.any():
+        if np.any(ar[pm] != 2):
+            raise ValueError("pmm pools must have 2 tokens")
+        keys.append((_lib.KIND_PMM, 2, np.nonzero(pm)[0]))
     cs = hp.kind == KIND_CRYPTOSWAP_HOST
     if cs.any():
         if np.any((ar[cs] != 2) & (ar[cs] != 3)):
@@ -1289,6 +1450,8 @@ class DeviceBucket:
             self.logrw = torch.as_tensor(_padded(P, self.stride, 0.0), **f64)
         if self.kind == _lib.KIND_ECLP:                    # (alpha, beta, c, s, lam, r, p) in seven weights rows
             self.weights = torch.as_tensor(_padded(np.asarray(hp.eclp, np.float64)[spec.sel].T, self.stride, 1.0), **f64)
+        if self.kind == _lib.KIND_PMM:                     # (pi, k, B0, Q0) in four weights rows
+            self.weights = torch.as_tensor(_padded(np.asarray(hp.pmm, np.float64)[spec.sel].T, self.stride, 1.0), **f64)
         if self.kind in (_lib.KIND_SUM, _lib.KIND_BINS):
             self.theta_bar = torch.zeros((2, self.stride), **f64)
         self.delta = self.lam = self.hcoef = self.hmask = None
@@ -1311,14 +1474,16 @@ class DeviceBucket:
     def write_update(self, loc: np.ndarray, R: Optional[np.ndarray], gamma: Optional[np.ndarray],
                      W: Optional[np.ndarray] = None, amp: Optional[np.ndarray] = None, sc: Optional[np.ndarray] = None,
                      rates: Optional[np.ndarray] = None, AD: Optional[np.ndarray] = None,
-                     cgam: Optional[np.ndarray] = None, eclp_st: Optional[np.ndarray] = None):
+                     cgam: Optional[np.ndarray] = None, eclp_st: Optional[np.ndarray] = None,
+                     pmm: Optional[np.ndarray] = None):
         """New reserves R (arity, n) and / or fees (n,) of the bucket-local pools `loc` (values already checked).
         Weighted pools also get logrw = log(R / W) with their weights W (arity, n), the expression of __init__;
         StableSwap pools get the invariant D of the new reserves from their rates W and amplification amp (n,), or, when
         their A or rates change, the new rates (arity, n) in the weights rows and AD = (A, D) (2, n) in logrw rows 0-1;
         cryptoswap pools likewise, with their curve gammas cgam (n,), and AD = (A, G, D) (3, n) in logrw rows 0-2;
         concentrated pools get their new (s, c) from sc (2, n), with R their derived reserves (ladder_state); E-CLPs
-        get the state (r, p) of their new reserves from eclp_st (2, n) in weights rows 5-6."""
+        get the state (r, p) of their new reserves from eclp_st (2, n) in weights rows 5-6; PMM pools get their new
+        (pi, k, B0, Q0) (4, n) from pmm in the four weights rows."""
         f64 = dict(dtype=torch.float64, device=self._device)
         li = torch.as_tensor(loc, dtype=torch.int64, device=self._device)
         if sc is not None:
@@ -1335,6 +1500,8 @@ class DeviceBucket:
                 self.logrw[:, li] = torch.as_tensor(np.log(R / W), **f64)
         if eclp_st is not None:
             self.weights[5:7, li] = torch.as_tensor(eclp_st, **f64)
+        if pmm is not None:
+            self.weights[:, li] = torch.as_tensor(pmm, **f64)
         if rates is not None:
             self.weights[:, li] = torch.as_tensor(rates, **f64)
         if AD is not None:
@@ -1824,6 +1991,8 @@ class PoolStore:
         self._amp_host = hp.amp                                          # StableSwap / cryptoswap amplification
         self._cgam_host = hp.cgam                                        # cryptoswap curve gamma
         self._eclp_host = hp.eclp                                        # E-CLP parameters (immutable; state on the device)
+        self._pmm_host = hp.pmm                                          # PMM (pi, k, B0, Q0) (copied at the first update)
+        self._own_pmm = False
         self._own_stable = False                                         # weights / amp are this store's copies
         self._lad_host = (hp.lad_ptr, hp.lad_rec)                        # concentrated records
         self._lad = None                                                 # LadderSlab
@@ -1890,7 +2059,7 @@ class PoolStore:
         token ids, rates, gamma, A, D), 80 B per concentrated pool (token ids, gamma, (s, c, first record, T), and the b_c,
         L_c, b_{c+1} and end bound the kernel reads for a trade inside the current interval; one that crosses bounds
         reads O(log) records more), 88 B per E-CLP pool (reserves, token ids, gamma, its seven parameters and state),
-        + nu, psi, arb."""
+        64 B per PMM pool (reserves, token ids, gamma, (pi, k, B0, Q0)), + nu, psi, arb."""
         n = 0
         for b in self.buckets:
             n += b.m * (28 * b.arity + 12 if b.kind == _lib.KIND_GEOMEAN else 48 if b.kind == _lib.KIND_BOUNDED
@@ -1899,6 +2068,7 @@ class PoolStore:
                         else 72 if b.kind == _lib.KIND_CRYPTOSWAP
                         else 148 if b.kind == _lib.KIND_CRYPTOSWAP_3
                         else 88 if b.kind == _lib.KIND_ECLP
+                        else 64 if b.kind == _lib.KIND_PMM
                         else 20 * b.arity + 24 if b.kind == _lib.KIND_STABLESWAP_N else 32)
         return n + 16 * self.n_tokens + 8
 
@@ -2050,7 +2220,7 @@ class PoolStore:
         return _bin_fills(self._bins().records(i), int(z), g, t)
 
     def update_pools(self, pool_ids, reserves=None, fees=None, prices=None, ladders=None, amp=None, rates=None,
-                     curve_gamma=None, bins=None):
+                     curve_gamma=None, bins=None, pmm=None):
         """Set new reserves, fees, prices, ladders, bins, A and / or rates of some pools in place: the store then
         equals, bit for bit, a PoolStore built from a HostPools of the updated literals, without re-uploading the pools or
         rebuilding the blocked layout (which depends on the token ids only).  pool_ids: global pool indices (the order of
@@ -2080,7 +2250,10 @@ class PoolStore:
         fresh pool's.  A bins pool takes no reserves= (its reserves are derived from its bins).  store.bin_fills(i, t)
         splits a trade over the pool's current bins.  E-CLP pools take reserves= and fees=: their state (r, p) is
         recomputed with eclp_state, as HostPools does; their parameters are structure (immutable on chain: a changed
-        pool is a new store).
+        pool is a new store).  PMM pools take reserves= (a swap: pi, k and the long side's target are kept, the short
+        side's target is re-derived with pmm_targets, as HostPools does), fees= and pmm=: pmm[k] = (pi, k, B0, Q0), the
+        pool's whole new row as from_lists takes it (a DPP reset, a deposit or a withdrawal; with reserves= for the
+        new balances, else on the current ones), the target rule applied as from_lists does.  Both sides short raises.
 
         All or nothing: bad ids (out of range, repeated), lengths or values (the rules of HostPools.from_lists and
         validate) raise ValueError before anything is written on the device or in the store's host state, and so does an
@@ -2094,7 +2267,7 @@ class PoolStore:
             store.update_pools(ids, reserves=new_R, fees=new_gamma)
             res = solve_pools(hp, utility, store=store, nu0=res.nu)"""
         u = check_pool_update(self.pool_ptr, self._kind_host, self._weights_host, pool_ids, reserves, fees, prices,
-                              ladders, amp, rates, curve_gamma, bins)
+                              ladders, amp, rates, curve_gamma, bins, pmm)
         bi, loc = self._pool_map()
         owner = bi[u.ids]
         plan = []
@@ -2140,6 +2313,10 @@ class PoolStore:
                 if not bool(np.all(np.isfinite(est[0]) & (est[0] > 0))):
                     raise ValueError("eclp invariant r must be finite and > 0 (balances out of fp64 range?)")
                 sc = est
+            if b.kind == _lib.KIND_PMM and (R is not None or u.pmm is not None):   # rows after the target rule
+                rows = u.pmm[e] if u.pmm is not None else np.asarray(self._pmm_host, np.float64)[ids]
+                Rd = R if R is not None else b.reserves[:, torch.as_tensor(loc[ids], device=self.device)].cpu().numpy()
+                sc = pmm_targets(Rd.T, rows).T
             plan.append((b, loc[ids], R, g, rs, ids, sc, lad, rt, AD))
         # the blocked bucket first: it checks its entries on the device and writes nothing if one is invalid
         rebuilt = 0
@@ -2158,11 +2335,18 @@ class PoolStore:
             if b.kind == _lib.KIND_ECLP:
                 b.write_update(l, R, g, eclp_st=sc)
                 continue
+            if b.kind == _lib.KIND_PMM:
+                b.write_update(l, R, g, pmm=sc)
+                continue
             b.write_update(l, R, g, W, amp_, sc, None if u.rates is None else rt, AD, cg_)
         # the store's host state, once the device holds the update
         for b, l, R, g, rs, ids, sc, lad, rt, AD in plan:
             if lad is not None:
                 (self._bins() if b.kind == _lib.KIND_BINS else self._ladders()).replace(ids, lad[0], lad[1])
+            if b.kind == _lib.KIND_PMM and sc is not None:
+                if not self._own_pmm:
+                    self._pmm_host, self._own_pmm = np.array(self._pmm_host, np.float64), True
+                self._pmm_host[ids] = sc.T
             if AD is not None:
                 if not self._own_stable:
                     self._weights_host, self._amp_host = self._weights_host.copy(), self._amp_host.copy()

@@ -112,7 +112,18 @@ enum {
                               the price p of the reserves (pools.eclp_state); reserves [2][stride] = (x, y), paid out
                               exactly at a cap.  logrw is not read.  hcoef is per pool, as for every pair kind:
                               r lam^2 nu1 p*^2 / h(p*)^3 (over gamma when tendering token 1), 0 at a cap.  Smooth: no
-                              theta_bar.  The evaluation has no TMA-staged kernel.                                     */
+                              theta_bar.  The evaluation has no TMA-staged kernel.                                     */,
+    CFMM_KIND_PMM = 12        /* DODO proactive market maker: guide price pi > 0 (token 1 per token 0), slippage factor
+                              0 < k <= 1, targets B0, Q0 > 0.  Base short (b <= B0): q - Q0 = pi d (1 + k d / b), d =
+                              B0 - b, marginal price pi (1 - k + k B0^2 / b^2); quote short (q <= Q0): the mirror (b <->
+                              q, B0 <-> Q0, pi -> 1 / pi).  The pool keeps (b, q) on or above this convex curve; its
+                              price runs over (0, inf), so it has no cap.  Not in the reference; arity 2 (any other
+                              arity: CFMM_E_KIND).  weights [4][stride] = (pi, k, B0, Q0) with the reserves on the curve
+                              (the adjusted-target rule, pools.pmm_targets: B < B0 and Q >= Q0, Q < Q0 and B >= B0,
+                              or (B, Q) = (B0, Q0)); reserves [2][stride] = (B, Q).  logrw is not read.  hcoef per pool, as for every
+                              pair kind: n1 p*^2 b* / (2 (k pi + p* - pi)) for p* >= pi, n1 pi q* / (2 (k p* + pi -
+                              p*)) below, over gamma when tendering token 1.  Smooth: no theta_bar.  The evaluation has
+                              no TMA-staged kernel.                                                                    */
 };
 
 enum {
@@ -135,7 +146,7 @@ typedef struct cfmm_bucket {
     const int32_t* tok_idx;
     const double* gamma;
     const double* weights;   /* GEOMEAN weights; BOUNDED_PRODUCT offsets; STABLESWAP(_N) rates; CONCENTRATED, BINS records;
-                                ECLP (alpha, beta, c, s, lam, r, p) */
+                                ECLP (alpha, beta, c, s, lam, r, p); PMM (pi, k, B0, Q0) */
     const double* logrw;     /* GEOMEAN log(R/w); STABLESWAP(_N) (A, D); CONCENTRATED (s, c, first record, T);
                                 BINS (first record, nb, z, p_ref) */
     const double* theta_bar; /* SUM and BINS only */
@@ -441,8 +452,8 @@ typedef struct cfmm_csr_pools {
     const double* gamma;       /* [n_pools] fees, arbitrage.py:22-28                                 */
     const uint8_t* kind;       /* [n_pools] CFMM_KIND_SUM | CFMM_KIND_BOUNDED_PRODUCT | CFMM_KIND_STABLESWAP |
                                             CFMM_KIND_CONCENTRATED | CFMM_KIND_CRYPTOSWAP |
-                                            CFMM_KIND_CRYPTOSWAP_3 | CFMM_KIND_BINS | CFMM_KIND_ECLP, else weighted
-                                            geometric mean                                           */
+                                            CFMM_KIND_CRYPTOSWAP_3 | CFMM_KIND_BINS | CFMM_KIND_ECLP |
+                                            CFMM_KIND_PMM, else weighted geometric mean              */
 } cfmm_csr_pools;
 
 typedef struct cfmm_batch {
@@ -518,6 +529,13 @@ int cfmm_batch_solve_bins(const cfmm_csr_pools* pools, const double* records, co
  * registers.  Same limits and workspace. */
 int cfmm_batch_solve_eclp(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
                           const cfmm_batch_params* prm, void* work, void* stream);
+/* The same solve for pool sets that hold CFMM_KIND_PMM pools, beside every kind cfmm_batch_solve_eclp takes (the eight
+ * entry points above give their problems status 3).  In the CSR arrays a PMM pool carries (B, Q) in its reserves and, in
+ * its first logrw slot, the index r_i of its record in `records` (units of 4 f64): records[4 r_i .. 4 r_i + 3] = {pi, k,
+ * B0, Q0}, after the E-CLP pools' records in the same buffer (CFMM_E_NULL if NULL).  A ninth kernel instance, so the
+ * others keep their registers.  Same limits and workspace. */
+int cfmm_batch_solve_pmm(const cfmm_csr_pools* pools, const double* records, const cfmm_batch* batch,
+                         const cfmm_batch_params* prm, void* work, void* stream);
 
 /*
  * All-reduce (sum) of n doubles over NVLink peer memory, the ONE collective of a pool-sharded dual evaluation (SURVEY
